@@ -782,7 +782,8 @@ static PFN_tmapEncodeTiled get_encode_fn() {
 
 // elem_bytes: 2 (fp16) or 4 (fp32); strides in elements
 static int make_tmap(CUtensorMap* tm, const void* base, int elem_bytes, int rank, const uint64_t* dims,
-                     const uint64_t* strides_elems, const uint32_t* box, const char* what) {
+                     const uint64_t* strides_elems, const uint32_t* box, const char* what,
+                     CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   PFN_tmapEncodeTiled enc = get_encode_fn();
   if (!enc) return fail(T2H_ECUDA, "cuTensorMapEncodeTiled entry point unavailable");
   cuuint64_t gdim[5], gstr[5];
@@ -802,7 +803,7 @@ static int make_tmap(CUtensorMap* tm, const void* base, int elem_bytes, int rank
     return fail(T2H_EINVAL, "%s: base pointer not 16-byte aligned", what);
   CUresult r = enc(tm, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32,
                    rank, const_cast<void*>(base), gdim, gstr, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                   swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return fail(T2H_ECUDA,
@@ -868,9 +869,13 @@ static int launch_swap(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
     }
     Q.debug = dbg;
   }
-  Q.a_slots = 3;
-  int nb = (C::kRingBytes - Q.a_slots * C::kASlot) / C::kBSlot;
+  // ring depths from what the register epilogue leaves of the shared memory: 4 A slabs load the next chunk's hi and
+  // lo slabs during the whole current chunk, the rest holds weight tiles (4: two taps of the 3-product order ahead).
+  // The kernel's ring invariant needs a_slots >= 3 and b_slots >= 2.
+  Q.a_slots = 4;
+  int nb = (kSwapRingBytes - Q.a_slots * C::kASlot) / C::kBSlot;
   Q.b_slots = nb > kMaxSlots ? kMaxSlots : nb;
+  if (Q.b_slots < 2) return fail(T2H_EINVAL, "tapgemm: shared-memory rings do not fit");
   int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
   T2H_CUDA(launch_pdl(tapgemm_swap_kernel<MBLK, FUSE>, dim3(grid), dim3(kSwapThreads), kDynSmem, stream, 1, tmA, tmB,
                       tmD, tmR, Q));
@@ -1136,12 +1141,17 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
     uint64_t dims[4] = {(uint64_t)p->n_out, (uint64_t)p->W, (uint64_t)p->H, imgs};
     uint64_t str[4] = {1, sw, sh, sn};
     uint32_t box[4] = {(uint32_t)(esz == 4 ? 32 : 64), (uint32_t)TW, (uint32_t)TH, 1};
-    if (swap) box[2] = (uint32_t)(32 / TW);  // one warp's 32 pixels
-    int rc = make_tmap(&tmD, p->d, esz, 4, dims, str, box, "tapgemm D");
+    CUtensorMapSwizzle sw_mode = CU_TENSOR_MAP_SWIZZLE_128B;
+    if (swap) {  // one box of a swapped-kernel warp: 16 channels (64 bytes) x 32 pixels
+      box[0] = 16;
+      box[2] = (uint32_t)(32 / TW);
+      sw_mode = CU_TENSOR_MAP_SWIZZLE_64B;
+    }
+    int rc = make_tmap(&tmD, p->d, esz, 4, dims, str, box, "tapgemm D", sw_mode);
     if (rc) return rc;
     if (p->residual) {
       uint64_t rdims[4] = {(uint64_t)p->n_out, (uint64_t)p->W, (uint64_t)p->H, (uint64_t)p->n_img};
-      rc = make_tmap(&tmR, p->residual, 4, 4, rdims, str, box, "tapgemm residual");
+      rc = make_tmap(&tmR, p->residual, 4, 4, rdims, str, box, "tapgemm residual", sw_mode);
       if (rc) return rc;
     }
   }

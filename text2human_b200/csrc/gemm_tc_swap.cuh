@@ -6,19 +6,68 @@
 // operand, so D^T[cout, pixel] accumulates with one output channel per accumulator row.  That is the
 // layout the per-channel epilogue wants: bias, GroupNorm sums and norm-backward sums are per lane.
 //
-// Epilogue: staging row = output channel, staging column = pixel.  Each of the 8 consumer warps owns 32
-// channels = one 128-byte row segment of the NHWC output and alternate 32-pixel chunks, and works
-// independently (no block barriers): 32 pixels from the staging array -> +bias (per lane) -> +residual
-// (its own TMA-loaded 4 KB tile) -> GroupNorm partial sums (two registers per thread) -> conflict-free
-// transposed st.shared into a swizzled [32 pixels][32 channels] tile -> its own TMA store.
+// Mainloop: one MMA group (four K=16 steps of one (weight tile, slab view) product) stays in flight while the next
+// is issued; the ring slots a group read last are released once the following group has been issued and the
+// group itself has completed (wgmma.wait_group 1).
+//
+// Epilogue, straight from the accumulator registers: thread t of warpgroup wg holds output channels
+// 64 wg + 16 (t / 32) + (t % 32) / 4 and that + 8, at pixels 8 j + 2 (t % 4) + {0, 1} of every 8-pixel block j, so
+// each consumer warp owns 16 channels x 128 pixels and finishes them alone (no block or warpgroup barrier):
+// +bias (two registers) -> activation -> +residual (its own TMA-loaded boxes) -> GroupNorm / norm-backward partial
+// sums (per thread, reduced over the four lanes of a channel and the channels of a group) -> st.shared into its own
+// 64-byte-swizzled [32 pixels][16 channels] boxes -> TMA store.
 #pragma once
 
 namespace t2h {
 
-constexpr int kWarpTile = 32 * 128;  // 32 pixels x 32 fp32 channels
-
-constexpr int kSwapThreads = 384;  // 4 producer warps + 8 consumer warps (two per 32-channel quarter)
+constexpr int kSwapThreads = 384;  // 4 producer warps + 8 consumer warps (two warpgroups of 64 output channels)
 constexpr int kFuseThreads = 96;   // FUSE: warps 0-2 build the activation slabs
+constexpr int kSwapBox = 32 * 16 * 4;         // one TMA box of the epilogue: 32 pixels x 16 fp32 channels
+constexpr int kSwapWarpBuf = 4 * kSwapBox;    // a consumer warp's 128 pixels: residual in, output out, in place
+static_assert(8 * kSwapWarpBuf == kEpiBytes, "epilogue boxes");
+constexpr int kSwapRingBytes = kDynSmem - 1024 - kEpiBytes;  // A ring + B ring
+// Register split (setmaxnreg): the producer warpgroup only issues TMA and waits on barriers; the consumers hold a
+// 64-register accumulator plus the epilogue's values.  The split redistributes what the CTA was launched with, 384
+// threads x 168 registers (the __launch_bounds__ ceiling): 128 x 40 + 256 x 232.  The fused GroupNorm producer does
+// real arithmetic in warps 0-2 and keeps more: 128 x 104 + 256 x 200.
+template <bool FUSE>
+struct SwapRegs {
+  static constexpr int kProducer = FUSE ? 104 : 40;
+  static constexpr int kConsumer = FUSE ? 200 : 232;
+  static_assert(128 * kProducer + 256 * kConsumer <= kSwapThreads * 168, "register split exceeds the CTA's registers");
+};
+
+// byte offset of fp32 channel c (0..15) of pixel i (0..31) in a [32][16] box TMA wrote with the 64-byte swizzle
+// (address bits [4,6) ^= bits [7,9))
+__device__ __forceinline__ int swz64(int i, int c) {
+  const int o = i * 64 + c * 4;
+  return o ^ ((o >> 3) & 0x30);
+}
+
+// norm-backward: add a thread's per-channel sums (channels c and c + 8) to nb_sums, after reducing them over the
+// four lanes that hold the same channel
+__device__ __forceinline__ void nb_flush(const TapGemmDev& P, int img, int c, int lane, float s1a, float s1b, float s2a,
+                                         float s2b) {
+#pragma unroll
+  for (int off = 1; off < 4; off <<= 1) {
+    s1a += __shfl_xor_sync(0xffffffffu, s1a, off);
+    s1b += __shfl_xor_sync(0xffffffffu, s1b, off);
+    s2a += __shfl_xor_sync(0xffffffffu, s2a, off);
+    s2b += __shfl_xor_sync(0xffffffffu, s2b, off);
+  }
+  if ((lane & 3) == 0) {
+    if (c < P.n_out) {
+      double* dst = P.nb_sums + ((long long)img * P.n_out + c) * 2;
+      atomicAdd(dst, (double)s1a);
+      atomicAdd(dst + 1, (double)s2a);
+    }
+    if (c + 8 < P.n_out) {
+      double* dst = P.nb_sums + ((long long)img * P.n_out + c + 8) * 2;
+      atomicAdd(dst, (double)s1b);
+      atomicAdd(dst + 1, (double)s2b);
+    }
+  }
+}
 
 // FUSE = true: the activation operand is NOT read as fp16 planes by TMA.  The kernel takes the fp32 NHWC tensor the
 // previous conv wrote plus its GroupNorm statistics, and three producer warps (0-2) build the swizzled hi / lo slabs
@@ -26,14 +75,21 @@ constexpr int kFuseThreads = 96;   // FUSE: warps 0-2 build the activation slabs
 // swish -> fp16 split -> st.shared in the 128-byte-swizzle image a TMA box would have produced.  This is
 // Normalize() + nonlinearity() (vqgan_arch.py:510-517) folded into the consuming conv: the gn_apply pass and its
 // 8 bytes per element of HBM traffic disappear.  Same arithmetic, same order as gn_apply_kernel -> identical slabs.
+//
+// Ring invariant: no group waits on a slot whose release is deferred behind it.  When a group's operands are waited
+// for, every slot whose last reader is two or more groups back has been released.  Each group reads one B tile and
+// the B index advances by at most one per group, so the tile a group needs reuses a slot released two groups back
+// whenever b_slots >= 2.  A slabs (3-product order hi.lo, hi.hi, lo.hi per tap): the next chunk's hi slab reuses the
+// slot of the current chunk's hi slab (last read by the hi.hi group before the chunk's final group) when
+// a_slots >= 2; the FUSE producer claims a chunk's hi and lo slots together before it marks either full, so it also
+// needs the current chunk's lo slot's predecessor free: a_slots >= 3.  1-product: one slab per chunk, a_slots >= 2.
 template <int MBLK, bool FUSE>
 __global__ void __launch_bounds__(kSwapThreads, 1)
 tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
                     const __grid_constant__ TapGemmDev P) {
   using C = Cfg<128, MBLK>;
-  constexpr int NPIX = MBLK * 128;  // pixels per tile = wgmma N
-  constexpr int LD = C::kStageLd;
+  static_assert(MBLK == 1, "the register epilogue covers 128-pixel tiles");
   pdl_launch_dependents();  // the next kernel may start its prologue once every CTA of this one is running
   const int NA = P.a_slots, NB = P.b_slots;
   extern __shared__ uint8_t smem_raw[];
@@ -41,9 +97,7 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_ring = smem;
   uint8_t* b_ring = smem + NA * C::kASlot;
-  uint8_t* out_buf = b_ring + NB * C::kBSlot;     // 8 warps x 4 KB
-  uint8_t* res_buf = out_buf + 2 * kEpiBufBytes;  // 8 warps x 4 KB
-  float* const stage = reinterpret_cast<float*>(res_buf + 2 * kEpiBufBytes);  // [128 couts][LD] accumulator
+  uint8_t* epi_buf = b_ring + NB * C::kBSlot;  // 8 consumer warps x kSwapWarpBuf
 
   __shared__ __align__(8) uint64_t a_full[kMaxSlots];
   __shared__ __align__(8) uint64_t a_empty[kMaxSlots];
@@ -88,176 +142,203 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   const int a_planes = (P.nterms == 3) ? 2 : 1;
   const int slab_bytes = P.slab_rows * P.TW * 128;
 
-  if (FUSE && warp < 3) {
-    // ---------------------------------------------- activation slab producers: GroupNorm + swish + fp16 split
-    const int pt = threadIdx.x;  // 0..kFuseThreads-1
-    float* s_scale = gn_tab;
-    float* s_shift = gn_tab + 256;
-    const int tw_shift = 31 - __clz(P.TW);
-    const int R = P.slab_rows * P.TW;  // pixels of one slab
-    const int units = R * 8;           // 8 channels (one 16-byte smem chunk) each
-    const int cpg = P.C / P.ag_groups;
-    const double cnt = (double)P.ag_hw * cpg;
-    int cur_img = -1;
-    int sa = 0, pa = 0;
-    for (int tile = tile_first; tile < tile_end; tile += tile_step) {
-      const TileCoord t = decode_tile(P, tile, MBLK, 128);
-      if (t.img != cur_img) {
-        named_bar_sync(3, kFuseThreads);  // nobody still reads the previous image's table
-        for (int c = pt; c < P.C; c += kFuseThreads) {
-          const int g = c / cpg;
-          const double su = P.ag_stats[((long long)t.img * P.ag_groups + g) * 2 + 0];
-          const double sq = P.ag_stats[((long long)t.img * P.ag_groups + g) * 2 + 1];
-          const double mean = su / cnt;
-          double var = sq / cnt - mean * mean;
-          if (var < 0) var = 0;
-          const float rstd = (float)(1.0 / sqrt(var + (double)P.ag_eps));
-          const float ga = P.ag_gamma[c] * rstd;
-          s_scale[c] = ga;
-          s_shift[c] = P.ag_beta[c] - (float)mean * ga;
-        }
-        named_bar_sync(3, kFuseThreads);
-        cur_img = t.img;
-      }
-      const float* ximg = P.ax + (long long)t.img * P.ax_sn;
-      for (int g = 0; g < P.ngroups; ++g) {
-        const int h_base = t.h0 + P.g_dy0[g], w_base = t.w0 + P.g_dx[g];
-        for (int ch = 0; ch < P.kchunks; ++ch) {
-          const int s_hi = sa;
-          mbar_wait(&a_empty[sa], pa ^ 1);
-          if (++sa == NA) { sa = 0; pa ^= 1; }
-          int s_lo = -1;
-          if (a_planes == 2) {
-            s_lo = sa;
-            mbar_wait(&a_empty[sa], pa ^ 1);
-            if (++sa == NA) { sa = 0; pa ^= 1; }
-          }
-          uint8_t* hi_base = a_ring + s_hi * C::kASlot;
-          uint8_t* lo_base = a_ring + (s_lo >= 0 ? s_lo : s_hi) * C::kASlot;
-          const int c0 = ch * kBK;
-#pragma unroll 4
-          for (int u = pt; u < units; u += kFuseThreads) {
-            const int r = u >> 3, j = u & 7;
-            const int h = h_base + (r >> tw_shift), w = w_base + (r & (P.TW - 1));
-            const bool ok = (h >= 0) && (h < P.ag_H) && (w >= 0) && (w < P.ag_W);
-            const float* src = ximg + (long long)h * P.ax_sh + (long long)w * P.ax_sw + c0 + j * 8;
-            float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
-            if (ok) {
-              v0 = __ldg(reinterpret_cast<const float4*>(src));
-              v1 = __ldg(reinterpret_cast<const float4*>(src) + 1);
-            }
-            const float f[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-            __align__(16) __half hh[8];
-            __align__(16) __half ll[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              float y = 0.f;
-              if (ok) {   // conv zero padding applies to the NORMALISED activation: outside pixels stay 0
-                y = f[e] * s_scale[c0 + j * 8 + e] + s_shift[c0 + j * 8 + e];
-                if (P.ag_swish) y = y / (1.0f + __expf(-y));
-              }
-              split_f16(y, hh[e], ll[e]);
-            }
-            *reinterpret_cast<uint4*>(hi_base + swz(r, j)) = *reinterpret_cast<const uint4*>(hh);
-            if (s_lo >= 0) *reinterpret_cast<uint4*>(lo_base + swz(r, j)) = *reinterpret_cast<const uint4*>(ll);
-          }
-          fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core's async proxy
-          named_bar_sync(3, kFuseThreads);
-          if (pt == 0) {
-            mbar_arrive(&a_full[s_hi]);
-            if (s_lo >= 0) mbar_arrive(&a_full[s_lo]);
-          }
-        }
-      }
-    }
-  } else if (!FUSE && warp == 0) {
-    // ---------------------------------------------- activation slab producer
-    if (lane == 0) {
+  if (warp < 4) {
+    // (each role's setmaxnreg sits inside its branch: ptxas ignores a reallocation that code needing more registers
+    // can follow)
+    setmaxnreg_dec<SwapRegs<FUSE>::kProducer>();
+    if (FUSE && warp < 3) {
+      // ---------------------------------------------- activation slab producers: GroupNorm + swish + fp16 split
+      const int pt = threadIdx.x;  // 0..kFuseThreads-1
+      float* s_scale = gn_tab;
+      float* s_shift = gn_tab + 256;
+      const int tw_shift = 31 - __clz(P.TW);
+      const int R = P.slab_rows * P.TW;  // pixels of one slab
+      const int units = R * 8;           // 8 channels (one 16-byte smem chunk) each
+      const int cpg = P.C / P.ag_groups;
+      const double cnt = (double)P.ag_hw * cpg;
+      int cur_img = -1;
       int sa = 0, pa = 0;
       for (int tile = tile_first; tile < tile_end; tile += tile_step) {
         const TileCoord t = decode_tile(P, tile, MBLK, 128);
-        for (int g = 0; g < P.ngroups; ++g)
-          for (int ch = 0; ch < P.kchunks; ++ch)
-            for (int pl = 0; pl < a_planes; ++pl) {
+        if (t.img != cur_img) {
+          named_bar_sync(3, kFuseThreads);  // nobody still reads the previous image's table
+          for (int c = pt; c < P.C; c += kFuseThreads) {
+            const int g = c / cpg;
+            const double su = P.ag_stats[((long long)t.img * P.ag_groups + g) * 2 + 0];
+            const double sq = P.ag_stats[((long long)t.img * P.ag_groups + g) * 2 + 1];
+            const double mean = su / cnt;
+            double var = sq / cnt - mean * mean;
+            if (var < 0) var = 0;
+            const float rstd = (float)(1.0 / sqrt(var + (double)P.ag_eps));
+            const float ga = P.ag_gamma[c] * rstd;
+            s_scale[c] = ga;
+            s_shift[c] = P.ag_beta[c] - (float)mean * ga;
+          }
+          named_bar_sync(3, kFuseThreads);
+          cur_img = t.img;
+        }
+        const float* ximg = P.ax + (long long)t.img * P.ax_sn;
+        for (int g = 0; g < P.ngroups; ++g) {
+          const int h_base = t.h0 + P.g_dy0[g], w_base = t.w0 + P.g_dx[g];
+          for (int ch = 0; ch < P.kchunks; ++ch) {
+            const int s_hi = sa;
+            mbar_wait(&a_empty[sa], pa ^ 1);
+            if (++sa == NA) { sa = 0; pa ^= 1; }
+            int s_lo = -1;
+            if (a_planes == 2) {
+              s_lo = sa;
               mbar_wait(&a_empty[sa], pa ^ 1);
-              if (P.debug & 4) {
-                mbar_arrive(&a_full[sa]);
-              } else {
-                mbar_expect_tx(&a_full[sa], slab_bytes);
-                tma_load_4d(&tmA, &a_full[sa], a_ring + sa * C::kASlot, ch * kBK, t.w0 + P.g_dx[g],
-                            t.h0 + P.g_dy0[g], t.img + P.g_ioff[g] + pl * P.a_term_imgs);
-              }
-              if (++sa == NA) {
-                sa = 0;
-                pa ^= 1;
-              }
+              if (++sa == NA) { sa = 0; pa ^= 1; }
             }
-      }
-    }
-  } else if (warp == 3) {
-    // ---------------------------------------------- weight tile producer (128 couts x 64 k)
-    if (lane == 0) {
-      int sb = 0, pb = 0;
-      for (int tile = tile_first; tile < tile_end; tile += tile_step) {
-        const TileCoord t = decode_tile(P, tile, MBLK, 128);
-        for (int g = 0; g < P.ngroups; ++g)
-          for (int ch = 0; ch < P.kchunks; ++ch)
-            for (int tp = 0; tp < P.g_ntaps[g]; ++tp)
-              for (int pl = a_planes - 1; pl >= 0; --pl) {  // lo first, then hi
-                mbar_wait(&b_empty[sb], pb ^ 1);
-                if (P.debug & 4) {
-                  mbar_arrive(&b_full[sb]);
-                } else {
-                  mbar_expect_tx(&b_full[sb], C::kBSlot);
-                  tma_load_4d(&tmB, &b_full[sb], b_ring + sb * C::kBSlot, ch * kBK, t.n0,
-                              P.g_btap[g][tp] + pl * P.b_term_g, 0);
+            uint8_t* hi_base = a_ring + s_hi * C::kASlot;
+            uint8_t* lo_base = a_ring + (s_lo >= 0 ? s_lo : s_hi) * C::kASlot;
+            const int c0 = ch * kBK;
+  #pragma unroll 4
+            for (int u = pt; u < units; u += kFuseThreads) {
+              const int r = u >> 3, j = u & 7;
+              const int h = h_base + (r >> tw_shift), w = w_base + (r & (P.TW - 1));
+              const bool ok = (h >= 0) && (h < P.ag_H) && (w >= 0) && (w < P.ag_W);
+              const float* src = ximg + (long long)h * P.ax_sh + (long long)w * P.ax_sw + c0 + j * 8;
+              float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
+              if (ok) {
+                v0 = __ldg(reinterpret_cast<const float4*>(src));
+                v1 = __ldg(reinterpret_cast<const float4*>(src) + 1);
+              }
+              const float f[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+              __align__(16) __half hh[8];
+              __align__(16) __half ll[8];
+  #pragma unroll
+              for (int e = 0; e < 8; ++e) {
+                float y = 0.f;
+                if (ok) {   // conv zero padding applies to the NORMALISED activation: outside pixels stay 0
+                  y = f[e] * s_scale[c0 + j * 8 + e] + s_shift[c0 + j * 8 + e];
+                  if (P.ag_swish) y = y / (1.0f + __expf(-y));
                 }
-                if (++sb == NB) {
-                  sb = 0;
-                  pb ^= 1;
+                split_f16(y, hh[e], ll[e]);
+              }
+              *reinterpret_cast<uint4*>(hi_base + swz(r, j)) = *reinterpret_cast<const uint4*>(hh);
+              if (s_lo >= 0) *reinterpret_cast<uint4*>(lo_base + swz(r, j)) = *reinterpret_cast<const uint4*>(ll);
+            }
+            fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core's async proxy
+            named_bar_sync(3, kFuseThreads);
+            if (pt == 0) {
+              mbar_arrive(&a_full[s_hi]);
+              if (s_lo >= 0) mbar_arrive(&a_full[s_lo]);
+            }
+          }
+        }
+      }
+    } else if (!FUSE && warp == 0) {
+      // ---------------------------------------------- activation slab producer
+      if (lane == 0) {
+        int sa = 0, pa = 0;
+        for (int tile = tile_first; tile < tile_end; tile += tile_step) {
+          const TileCoord t = decode_tile(P, tile, MBLK, 128);
+          for (int g = 0; g < P.ngroups; ++g)
+            for (int ch = 0; ch < P.kchunks; ++ch)
+              for (int pl = 0; pl < a_planes; ++pl) {
+                mbar_wait(&a_empty[sa], pa ^ 1);
+                if (P.debug & 4) {
+                  mbar_arrive(&a_full[sa]);
+                } else {
+                  mbar_expect_tx(&a_full[sa], slab_bytes);
+                  tma_load_4d(&tmA, &a_full[sa], a_ring + sa * C::kASlot, ch * kBK, t.w0 + P.g_dx[g],
+                              t.h0 + P.g_dy0[g], t.img + P.g_ioff[g] + pl * P.a_term_imgs);
+                }
+                if (++sa == NA) {
+                  sa = 0;
+                  pa ^= 1;
                 }
               }
+        }
+      }
+    } else if (warp == 3) {
+      // ---------------------------------------------- weight tile producer (128 couts x 64 k)
+      if (lane == 0) {
+        int sb = 0, pb = 0;
+        for (int tile = tile_first; tile < tile_end; tile += tile_step) {
+          const TileCoord t = decode_tile(P, tile, MBLK, 128);
+          for (int g = 0; g < P.ngroups; ++g)
+            for (int ch = 0; ch < P.kchunks; ++ch)
+              for (int tp = 0; tp < P.g_ntaps[g]; ++tp)
+                for (int pl = a_planes - 1; pl >= 0; --pl) {  // lo first, then hi
+                  mbar_wait(&b_empty[sb], pb ^ 1);
+                  if (P.debug & 4) {
+                    mbar_arrive(&b_full[sb]);
+                  } else {
+                    mbar_expect_tx(&b_full[sb], C::kBSlot);
+                    tma_load_4d(&tmB, &b_full[sb], b_ring + sb * C::kBSlot, ch * kBK, t.n0,
+                                P.g_btap[g][tp] + pl * P.b_term_g, 0);
+                  }
+                  if (++sb == NB) {
+                    sb = 0;
+                    pb ^= 1;
+                  }
+                }
+        }
       }
     }
-  } else if (warp >= 4) {
+  } else {
     // ---------------------------------------------- consumers: D^T[cout, pixel] += W * slab^T, then the epilogue
+    setmaxnreg_inc<SwapRegs<FUSE>::kConsumer>();
     const int wg = (warp - 4) >> 2;  // output channels 64 wg .. 64 wg + 63 of the tile
-    const int wt = threadIdx.x & 127;
     const uint32_t row16 = (uint32_t)(P.TW * 128) >> 4;  // one slab image row, in 16-byte units
     const uint64_t x_desc0 = gmma_desc(smem_u32(a_ring));
     const uint64_t w_desc0 = gmma_desc(smem_u32(b_ring) + 8192u * wg);
     constexpr uint32_t A16 = C::kASlot >> 4, B16 = C::kBSlot >> 4;
     const int ngroups = P.ngroups, kchunks = P.kchunks;
     int sa = 0, pa = 0, sb = 0, pb = 0;
-    // every consumer thread arrives once the warpgroup's MMAs reading the slot have completed (a lane-0 arrival
-    // between wgmmas puts them on a divergent path, and ptxas then serialises every MMA)
-    auto release = [&](uint64_t* bar) { mbar_arrive(bar); };
-    const int q = warp & 3;
-    const int e = warp - 4;          // 0..7
-    const int half = e >> 2;         // which of the quadrant's two warps
-    uint8_t* my_out = out_buf + e * kWarpTile;
-    uint8_t* my_res = res_buf + e * kWarpTile;
+    const int e = warp - 4;  // 0..7
+    uint8_t* my_buf = epi_buf + e * kSwapWarpBuf;
+    const uint32_t buf_s = smem_u32(my_buf);
     const bool has_res = P.residual != nullptr;
-    const int tw_shift = 31 - __clz(P.TW);      // TW is a power of two <= 32
-    const int rows_per_chunk = 32 >> tw_shift;  // image rows covered by 32 pixels
-    constexpr int NCH = NPIX / 32;
+    const int tw_shift = 31 - __clz(P.TW);      // TW is a power of two <= 16
+    const int rows_per_box = 32 >> tw_shift;    // image rows covered by 32 pixels
+    const int m2 = 2 * (lane & 3);              // pixel offset of this thread inside each 8-pixel block
     uint32_t res_par = 0;
     const int cpg = P.gn_cpg;
-    const int red = cpg < 32 ? cpg : 32;  // lanes sharing a GroupNorm group inside this warp
-    const bool nb = P.nb_sums != nullptr;  // norm-backward sums: the "residual" tile is x and is not added
-    // (plain locals and an explicit flush at both sites: a by-reference lambda put the running sums in local memory)
-    float nb_mean = 0.f, nb_rstd = 0.f, nb_ga = 0.f, nb_be = 0.f, nb_s1 = 0.f, nb_s2 = 0.f;
-    int nb_img = -1, nb_c0 = -1;
+    const int red = 4 * (cpg < 8 ? cpg : 8);  // lanes holding one GroupNorm group's (channel, pixel) partial sums
+    // norm-backward sums: the "residual" tile is x and is not added (never with the fused producer: the host rejects it)
+    const bool nb = !FUSE && P.nb_sums != nullptr;
+    // per thread: channel c (index 0) and c + 8 (index 1); the sums run on across consecutive tiles of the same
+    // (image, channel block) and are flushed when that changes
+    float nb_mean[2] = {0.f, 0.f}, nb_rstd[2] = {0.f, 0.f}, nb_ga[2] = {0.f, 0.f}, nb_be[2] = {0.f, 0.f};
+    float nb_s1[2] = {0.f, 0.f}, nb_s2[2] = {0.f, 0.f};
+    int nb_img = -1, nb_c = -1;
 
     for (int tile = tile_first; tile < tile_end; tile += tile_step) {
+      const TileCoord t = decode_tile(P, tile, MBLK, 128);
+      const int c0 = t.n0 + 16 * e;       // this warp's 16 output channels
+      const int ca = c0 + (lane >> 2);    // this thread's channels: ca and ca + 8
+      if (has_res && lane == 0) {
+        // the tile's residual (or x) boxes load while its MMAs run, into the boxes the previous tile's output
+        // stores read from
+        tma_store_wait_read<0>();
+        mbar_expect_tx(&res_bar[e], kSwapWarpBuf);
+        for (int k = 0; k < 4; ++k)
+          tma_load_4d(&tmR, &res_bar[e], my_buf + k * kSwapBox, c0, t.w0, t.h0 + k * rows_per_box, t.img);
+        if (nb && tile + tile_step < tile_end) {
+          // the NEXT tile's x boxes go to L2 now, so that its loads above are L2 hits
+          const TileCoord tn = decode_tile(P, tile + tile_step, MBLK, 128);
+          for (int k = 0; k < 4; ++k)
+            tma_prefetch_4d(&tmR, tn.n0 + 16 * e, tn.w0, tn.h0 + k * rows_per_box, tn.img);
+        }
+      }
+      float acc[64];
       {
-        float acc[NPIX / 2];
         uint32_t accf = 0;
-        auto batch = [&](uint64_t w, uint64_t x) {
+        int rel_b = -1, rel_a = -1;  // the slots the group in flight is the last reader of (-1: none)
+        // every consumer thread arrives (a lane-0 arrival between wgmmas puts them on a divergent path, and ptxas
+        // then serialises every MMA); the arrivals are for the previous group, which wait_group 1 has completed
+        auto group = [&](uint64_t w, uint64_t x, int last_b, int last_a) {
           wgmma_fence();
           wgmma_chunk<0, 0>(acc, w, x, accf);
           wgmma_commit();
-          wgmma_wait<0>();
+          wgmma_wait<1>();
+          if (rel_b >= 0) mbar_arrive(&b_empty[rel_b]);
+          if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
+          rel_b = last_b;
+          rel_a = last_a;
         };
         for (int g = 0; g < ngroups; ++g) {
           const int nt = P.g_ntaps[g];
@@ -275,217 +356,189 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             const uint64_t xlo = x_desc0 + sa_lo * A16;
             for (int tp = 0; tp < nt; ++tp) {
               const uint32_t dy = tp == 0 ? dy0 : (tp == 1 ? dy1 : dy2);
+              const bool last = tp == nt - 1;
               if (a_planes == 1) {
                 mbar_wait(&b_full[sb], pb);
-                batch(w_desc0 + sb * B16, xhi + dy);
-                release(&b_empty[sb]);
+                group(w_desc0 + sb * B16, xhi + dy, sb, last ? sa_hi : -1);
                 if (++sb == NB) { sb = 0; pb ^= 1; }
               } else {
                 mbar_wait(&b_full[sb], pb);  // w_lo
-                batch(w_desc0 + sb * B16, xhi + dy);  // x_hi*w_lo
-                release(&b_empty[sb]);
+                group(w_desc0 + sb * B16, xhi + dy, sb, -1);  // x_hi*w_lo
                 if (++sb == NB) { sb = 0; pb ^= 1; }
                 mbar_wait(&b_full[sb], pb);  // w_hi
                 const uint64_t whi = w_desc0 + sb * B16;
-                batch(whi, xhi + dy);  // x_hi*w_hi
-                if (tp == nt - 1) release(&a_empty[sa_hi]);
+                group(whi, xhi + dy, -1, last ? sa_hi : -1);  // x_hi*w_hi
                 if (tp == 0) mbar_wait(&a_full[sa_lo], pa_lo);
-                batch(whi, xlo + dy);  // x_lo*w_hi
-                release(&b_empty[sb]);
+                group(whi, xlo + dy, sb, last ? sa_lo : -1);  // x_lo*w_hi
                 if (++sb == NB) { sb = 0; pb ^= 1; }
               }
             }
-            release(a_planes == 1 ? &a_empty[sa_hi] : &a_empty[sa_lo]);
           }
         }
+        wgmma_wait<0>();
         wgmma_fence_regs(acc);
-        named_bar_sync(4, 256);  // the previous tile's epilogue has read the staging array
-        acc_store_rows(acc, stage, LD, wg, wt);
-        named_bar_sync(4, 256);
+        if (rel_b >= 0) mbar_arrive(&b_empty[rel_b]);
+        if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
       }
-      const TileCoord t = decode_tile(P, tile, MBLK, 128);
-      const int c0 = t.n0 + q * 32;  // this warp's first output channel
-      const float bias_c =
-          (P.bias_mode == T2H_BIAS_COL && c0 + lane < P.n_out) ? __ldg(P.bias + t.img * P.bias_sn + c0 + lane) : 0.f;
-      auto issue_res = [&](int k) {
-        mbar_expect_tx(&res_bar[e], kWarpTile);
-        tma_load_4d(&tmR, &res_bar[e], my_res, c0, t.w0, t.h0 + k * rows_per_chunk, t.img);
-      };
-      if (has_res && lane == 0) issue_res(half);
-      constexpr int KSTEP = 2;  // chunks are dealt round-robin to the quadrant's warps
-      if (nb && lane == 0 && tile + tile_step < tile_end) {
-        // the NEXT tile's x boxes go to L2 now, while its MMAs run: the epilogue's own loads then cost an L2 hit
-        // instead of a DRAM round trip under load, four times per tile on the critical path
-        const TileCoord tn = decode_tile(P, tile + tile_step, MBLK, 128);
-        for (int k = half; k < NPIX / 32; k += KSTEP)
-          tma_prefetch_4d(&tmR, tn.n0 + q * 32, tn.w0, tn.h0 + k * rows_per_chunk, tn.img);
-      }
-      // interior tiles need no per-pixel validity test for the GroupNorm sums
-      const bool interior = (t.h0 + MBLK * P.TH <= P.H) && (t.w0 + P.TW <= P.W);
-      float gs = 0.f, gss = 0.f;
-      // norm-backward: this lane's channel constants of image t.img (mean, rstd from the forward statistics); the
-      // sums run on across consecutive tiles of the same (image, channel block) and are flushed when that changes
-      if (nb && (t.img != nb_img || c0 != nb_c0)) {
-        if (nb_img >= 0 && nb_c0 + lane < P.n_out) {
-          double* dst = P.nb_sums + ((long long)nb_img * P.n_out + nb_c0 + lane) * 2;
-          atomicAdd(dst, (double)nb_s1);
-          atomicAdd(dst + 1, (double)nb_s2);
-        }
-        nb_s1 = 0.f;
-        nb_s2 = 0.f;
-        nb_img = t.img;
-        nb_c0 = c0;
-        const int c = min(c0 + lane, P.n_out - 1);
-        const int ncpg = P.n_out / P.nb_groups;
-        const double cnt = (double)P.H * P.W * ncpg;
-        const double* st = P.nb_stats + ((long long)t.img * P.nb_groups + c / ncpg) * 2;
-        const double m = st[0] / cnt;
-        double var = st[1] / cnt - m * m;
-        if (var < 0) var = 0;
-        nb_mean = (float)m;
-        nb_rstd = (float)(1.0 / sqrt(var + (double)P.nb_eps));
-        nb_ga = __ldg(P.nb_gamma + c);
-        nb_be = __ldg(P.nb_beta + c);
-      }
-#pragma unroll 1
-      for (int k = half; k < NCH; k += KSTEP) {
-        uint32_t r[32];
-        stage_ld<32>(stage, LD, q * 32 + lane, k * 32, r);
-        if (P.debug & 1) {
-          if (has_res) {
-            mbar_wait(&res_bar[e], res_par);
-            res_par ^= 1;
-            __syncwarp();
-            if (lane == 0 && k + KSTEP < NCH) issue_res(k + KSTEP);
-          }
-          continue;
-        }
-        float v[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]) * P.alpha + bias_c;
-        if (P.act == T2H_ACT_GELU) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
-        } else if (P.act == T2H_ACT_RELU) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-        } else if (P.act == T2H_ACT_LRELU) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = v[i] > 0.f ? v[i] : 0.2f * v[i];
-        }
+      if (P.debug & 1) {
         if (has_res) {
           mbar_wait(&res_bar[e], res_par);
           res_par ^= 1;
-          if (nb) {
-            // v = dL/d act(norm(x)); accumulate pass 1 of the norm backward: sum du, sum du*xhat over the pixels.
-            // Pixels outside the image are zeroed up front (their x tile is zero-filled), the activation is chosen
-            // outside the element loop, two partial sums break the dependency chains.
-            if (!interior) {
-              const int hrow0 = t.h0 + k * rows_per_chunk;
+        }
+        continue;
+      }
+      // accumulator element i: channel ca + 8 ((i >> 1) & 1), pixel 8 (i >> 2) + m2 + (i & 1); in-box pixel and
+      // channel of the [32][16] box i >> 4
+      auto box_off = [&](int i) { return (i >> 4) * kSwapBox + swz64(8 * ((i >> 2) & 3) + m2 + (i & 1), (lane >> 2) + 8 * ((i >> 1) & 1)); };
+      auto pix_ok = [&](int i) {
+        const int p = 8 * (i >> 2) + m2 + (i & 1);
+        return (t.h0 + (p >> tw_shift) < P.H) && (t.w0 + (p & (P.TW - 1)) < P.W);
+      };
+      // interior tiles need no per-pixel validity test for the GroupNorm / norm-backward sums
+      const bool interior = (t.h0 + MBLK * P.TH <= P.H) && (t.w0 + P.TW <= P.W);
+      {
+        float bias2[2] = {0.f, 0.f};
+        if (P.bias_mode == T2H_BIAS_COL) {
+          if (ca < P.n_out) bias2[0] = __ldg(P.bias + t.img * P.bias_sn + ca);
+          if (ca + 8 < P.n_out) bias2[1] = __ldg(P.bias + t.img * P.bias_sn + ca + 8);
+        }
 #pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (!((hrow0 + (i >> tw_shift) < P.H) && (t.w0 + (i & (P.TW - 1)) < P.W))) v[i] = 0.f;
+        for (int i = 0; i < 64; ++i) acc[i] = acc[i] * P.alpha + bias2[(i >> 1) & 1];
+      }
+      if (P.act == T2H_ACT_GELU) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = gelu_erf(acc[i]);
+      } else if (P.act == T2H_ACT_RELU) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = fmaxf(acc[i], 0.f);
+      } else if (P.act == T2H_ACT_LRELU) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = acc[i] > 0.f ? acc[i] : 0.2f * acc[i];
+      }
+      if (has_res) {
+        mbar_wait(&res_bar[e], res_par);
+        res_par ^= 1;
+        if (nb) {
+          // norm-backward constants of this thread's two channels in image t.img (mean, rstd from the forward
+          // statistics); the previous (image, channel block)'s sums are flushed first
+          if (t.img != nb_img || c0 != nb_c) {
+            if (nb_img >= 0) nb_flush(P, nb_img, nb_c + (lane >> 2), lane, nb_s1[0], nb_s1[1], nb_s2[0], nb_s2[1]);
+            nb_img = t.img;
+            nb_c = c0;
+            const int ncpg = P.n_out / P.nb_groups;
+            const double cnt = (double)P.H * P.W * ncpg;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              nb_s1[h] = 0.f;
+              nb_s2[h] = 0.f;
+              const int c = min(ca + 8 * h, P.n_out - 1);
+              const double* st = P.nb_stats + ((long long)t.img * P.nb_groups + c / ncpg) * 2;
+              const double m = st[0] / cnt;
+              double var = st[1] / cnt - m * m;
+              if (var < 0) var = 0;
+              nb_mean[h] = (float)m;
+              nb_rstd[h] = (float)(1.0 / sqrt(var + (double)P.nb_eps));
+              nb_ga[h] = __ldg(P.nb_gamma + c);
+              nb_be[h] = __ldg(P.nb_beta + c);
             }
-            float s1b = 0.f, s2b = 0.f;
-            if (P.nb_act == 1) {
+          }
+          // acc = dL/d act(norm(x)); accumulate pass 1 of the norm backward: sum du, sum du*xhat over the pixels.
+          // Pixels outside the image are zeroed up front (their x boxes are zero-filled), the activation is chosen
+          // outside the element loop.
+          if (!interior) {
 #pragma unroll
-              for (int i = 0; i < 32; i += 2) {
-                const float x0 = *reinterpret_cast<const float*>(my_res + swz(i, lane >> 2) + ((lane & 3) << 2));
-                const float x1 = *reinterpret_cast<const float*>(my_res + swz(i + 1, lane >> 2) + ((lane & 3) << 2));
-                const float xh0 = (x0 - nb_mean) * nb_rstd, xh1 = (x1 - nb_mean) * nb_rstd;
-                const float du0 = v[i] * act_grad_fast(fmaf(xh0, nb_ga, nb_be), 1);
-                const float du1 = v[i + 1] * act_grad_fast(fmaf(xh1, nb_ga, nb_be), 1);
-                nb_s1 += du0; s1b += du1;
-                nb_s2 = fmaf(du0, xh0, nb_s2); s2b = fmaf(du1, xh1, s2b);
-              }
-            } else {
-              const int a = P.nb_act;
+            for (int i = 0; i < 64; ++i)
+              if (!pix_ok(i)) acc[i] = 0.f;
+          }
+          if (P.nb_act == 1) {
 #pragma unroll
-              for (int i = 0; i < 32; i += 2) {
-                const float x0 = *reinterpret_cast<const float*>(my_res + swz(i, lane >> 2) + ((lane & 3) << 2));
-                const float x1 = *reinterpret_cast<const float*>(my_res + swz(i + 1, lane >> 2) + ((lane & 3) << 2));
-                const float xh0 = (x0 - nb_mean) * nb_rstd, xh1 = (x1 - nb_mean) * nb_rstd;
-                const float du0 = v[i] * ((a == 2 && fmaf(xh0, nb_ga, nb_be) <= 0.f) ? 0.2f : 1.0f);
-                const float du1 = v[i + 1] * ((a == 2 && fmaf(xh1, nb_ga, nb_be) <= 0.f) ? 0.2f : 1.0f);
-                nb_s1 += du0; s1b += du1;
-                nb_s2 = fmaf(du0, xh0, nb_s2); s2b = fmaf(du1, xh1, s2b);
-              }
+            for (int i = 0; i < 64; ++i) {
+              const int h = (i >> 1) & 1;
+              const float xh = (lds_f32(buf_s + box_off(i)) - nb_mean[h]) * nb_rstd[h];
+              const float du = acc[i] * act_grad_fast(fmaf(xh, nb_ga[h], nb_be[h]), 1);
+              nb_s1[h] += du;
+              nb_s2[h] = fmaf(du, xh, nb_s2[h]);
             }
-            nb_s1 += s1b;
-            nb_s2 += s2b;
           } else {
+            const int a = P.nb_act;
 #pragma unroll
-            for (int i = 0; i < 32; ++i)  // row = pixel i, word = this lane's channel: conflict-free
-              v[i] += *reinterpret_cast<const float*>(my_res + swz(i, lane >> 2) + ((lane & 3) << 2));
-          }
-          __syncwarp();
-          if (lane == 0 && k + KSTEP < NCH) issue_res(k + KSTEP);  // overlaps the rest of this chunk
-        }
-        if (P.gn_stats) {
-          if (interior) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              gs += v[i];
-              gss = fmaf(v[i], v[i], gss);
-            }
-          } else {
-            const int hrow0 = t.h0 + k * rows_per_chunk;
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const bool ok = (hrow0 + (i >> tw_shift) < P.H) && (t.w0 + (i & (P.TW - 1)) < P.W);
-              const float x = ok ? v[i] : 0.f;
-              gs += x;
-              gss = fmaf(x, x, gss);
+            for (int i = 0; i < 64; ++i) {
+              const int h = (i >> 1) & 1;
+              const float xh = (lds_f32(buf_s + box_off(i)) - nb_mean[h]) * nb_rstd[h];
+              const float du = acc[i] * ((a == 2 && fmaf(xh, nb_ga[h], nb_be[h]) <= 0.f) ? 0.2f : 1.0f);
+              nb_s1[h] += du;
+              nb_s2[h] = fmaf(du, xh, nb_s2[h]);
             }
           }
-        }
-        if (P.epi_mode == EPI_DIRECT) {
-          // strided destination (NCHW conv_out, Cout < 128): the few valid channels store their pixels
-          const int c = c0 + lane;
-          if (c < P.n_out) {
-            float* dst = reinterpret_cast<float*>(P.d) + (long long)t.img * P.d_sn + (long long)c * P.d_sc;
-            const int hrow0 = t.h0 + k * rows_per_chunk;
+        } else {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const int h = hrow0 + (i >> tw_shift), w = t.w0 + (i & (P.TW - 1));
-              if (h < P.H && w < P.W) dst[(long long)h * P.d_sh + (long long)w * P.d_sw] = v[i];
-            }
-          }
-          continue;
-        }
-        if (lane == 0) tma_store_wait_read<0>();  // my_out's previous store has drained
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          *reinterpret_cast<float*>(my_out + swz(i, lane >> 2) + ((lane & 3) << 2)) = v[i];
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_4d(&tmD, my_out, c0, t.w0, t.h0 + k * rows_per_chunk, t.img);
-          tma_store_commit();
+          for (int i = 0; i < 64; ++i) acc[i] += lds_f32(buf_s + box_off(i));
         }
       }
       if (P.gn_stats) {
+        float gs[2] = {0.f, 0.f}, gss[2] = {0.f, 0.f};
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+          const float x = (interior || pix_ok(i)) ? acc[i] : 0.f;
+          gs[(i >> 1) & 1] += x;
+          gss[(i >> 1) & 1] = fmaf(x, x, gss[(i >> 1) & 1]);
+        }
+        // lanes 4c .. 4c + 3 hold channel c's pixels; the channels of a group are consecutive lane quads
         for (int off = 1; off < red; off <<= 1) {
-          gs += __shfl_xor_sync(0xffffffffu, gs, off);
-          gss += __shfl_xor_sync(0xffffffffu, gss, off);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            gs[h] += __shfl_xor_sync(0xffffffffu, gs[h], off);
+            gss[h] += __shfl_xor_sync(0xffffffffu, gss[h], off);
+          }
+        }
+        if (cpg >= 16) {  // channels ca and ca + 8 are in the same group
+          gs[0] += gs[1];
+          gss[0] += gss[1];
         }
         if ((lane & (red - 1)) == 0) {
-          const int g = (c0 + lane) / cpg;
-          double* dst = P.gn_stats + ((long long)t.img * P.gn_groups + g) * 2;
-          atomicAdd(dst, (double)gs);
-          atomicAdd(dst + 1, (double)gss);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (h == 1 && cpg >= 16) break;
+            double* dst = P.gn_stats + ((long long)t.img * P.gn_groups + (ca + 8 * h) / cpg) * 2;
+            atomicAdd(dst, (double)gs[h]);
+            atomicAdd(dst + 1, (double)gss[h]);
+          }
+        }
+      }
+      if (P.epi_mode == EPI_DIRECT) {
+        // strided destination (NCHW conv_out, Cout < 128): the threads of valid channels store their pixels
+        float* dst = reinterpret_cast<float*>(P.d) + (long long)t.img * P.d_sn;
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+          const int c = ca + 8 * ((i >> 1) & 1);
+          const int p = 8 * (i >> 2) + m2 + (i & 1);
+          const int h = t.h0 + (p >> tw_shift), w = t.w0 + (p & (P.TW - 1));
+          if (c < P.n_out && h < P.H && w < P.W) dst[(long long)c * P.d_sc + (long long)h * P.d_sh + (long long)w * P.d_sw] = acc[i];
+        }
+        continue;
+      }
+      // Output boxes, written in place of the residual boxes they were added from.  Per st.shared the 32 lanes
+      // write 8 channels x 4 pixels of one pixel parity; the 64-byte swizzle puts them on 16 banks, 2 lanes each:
+      // 2-way bank conflicts.
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        if (!has_res) {
+          if (lane == 0) tma_store_wait_read<3>();  // the store that last read this box (4 commits ago) is done
+          __syncwarp();
+        }
+#pragma unroll
+        for (int i = 16 * k; i < 16 * k + 16; ++i) sts_f32(buf_s + box_off(i), acc[i]);
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+          tma_store_4d(&tmD, my_buf + k * kSwapBox, c0, t.w0, t.h0 + k * rows_per_box, t.img);
+          tma_store_commit();
         }
       }
     }
-    if (nb && nb_img >= 0 && nb_c0 + lane < P.n_out) {
-      double* dst = P.nb_sums + ((long long)nb_img * P.n_out + nb_c0 + lane) * 2;
-      atomicAdd(dst, (double)nb_s1);
-      atomicAdd(dst + 1, (double)nb_s2);
-    }
+    if (nb && nb_img >= 0) nb_flush(P, nb_img, nb_c + (lane >> 2), lane, nb_s1[0], nb_s1[1], nb_s2[0], nb_s2[1]);
     if (lane == 0) tma_store_wait_read<0>();
   }
-
 }
 
 }  // namespace t2h
