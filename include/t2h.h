@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define T2H_VERSION 201
+#define T2H_VERSION 202
 
 #define T2H_OK 0
 #define T2H_EINVAL (-1)   /* bad argument / unsupported shape            */
@@ -152,18 +152,6 @@ typedef struct t2h_tapgemm_params {
                             ceil(C / 64)) STORES alpha*A.B to d + s*d_slab; t2h_splitk_reduce_ln sums the slabs in
                             a fixed order.  Single-image row GEMMs, no bias / act / residual                 */
   int64_t d_slab;        /* element distance between the k_partials slabs                                  */
-  /* Fused GroupNorm(+swish) activation operand (Normalize() + nonlinearity(), vqgan_arch.py:510-517, folded into the
-   * consuming 3x3 conv of ResnetBlock / conv_out, :599-609, :916-918, :1030-1032): when a_f32 != NULL the A operand is
-   * act(gn(a_f32)) computed on the fly from the fp32 NHWC tensor (strides a_sw/a_sh/a_sn in fp32 elements, extents
-   * a_H x a_W x C) and the statistics [n_img][groups][2] (sum, sumsq) its producer accumulated; `a` is ignored and
-   * nterms picks 1 or 3 products.  Spatial convs with Cout % 128 == 0 (or small strided Cout), C % 64 == 0, C <= 256. */
-  const float* a_f32;
-  const double* a_gn_stats;
-  const float* a_gn_gamma;
-  const float* a_gn_beta;
-  float a_gn_eps;
-  int32_t a_gn_swish;
-  int32_t a_gn_groups;
   /* Norm-backward sums in the epilogue (swapped-operand kernel: spatial convs with n_out % 128 == 0 and a plain fp32
    * NHWC destination): for a data-gradient conv whose output D is the gradient w.r.t. act(norm(x)*gamma+beta), with
    * nb_sums != NULL `residual` holds x (fp32, D's geometry; it is NOT added) and the epilogue accumulates

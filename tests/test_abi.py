@@ -31,33 +31,32 @@ def test_library_exports_every_declared_symbol():
     assert sorted(_lib.SIGNATURES) == names
 
 
-def test_version_and_error_string():
+def test_abi_version_matches_header_and_error_string():
+    """the library, the header's T2H_VERSION and the ctypes mirrors' ABI_VERSION agree"""
     lib = _lib.load()
-    assert lib.t2h_version() == 201
+    assert lib.t2h_version() == _lib.ABI_VERSION
+    assert re.search(r"#define T2H_VERSION (\d+)", open(HEADER).read()).group(1) == str(_lib.ABI_VERSION)
     assert isinstance(lib.t2h_last_error(), bytes)
 
 
 def test_struct_layout_matches_header():
-    code = r'''
-#include "t2h.h"
-#include <stdio.h>
-#include <stddef.h>
-int main(void){ printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\n", sizeof(t2h_tapgemm_params),
-  offsetof(t2h_tapgemm_params,b), offsetof(t2h_tapgemm_params,ntaps), offsetof(t2h_tapgemm_params,d),
-  offsetof(t2h_tapgemm_params,alpha), offsetof(t2h_tapgemm_params,gn_cpg),
-  sizeof(t2h_conv_wgrad_params), offsetof(t2h_conv_wgrad_params,x), offsetof(t2h_conv_wgrad_params,ntaps),
-  offsetof(t2h_conv_wgrad_params,dw), offsetof(t2h_conv_wgrad_params,k_split)); return 0; }
-'''
+    """sizeof and the offset of every field of both ctypes mirrors, against the C compiler's view of the header"""
+    structs = {"t2h_tapgemm_params": _lib.TapGemmParams, "t2h_conv_wgrad_params": _lib.ConvWgradParams}
+    prints, want = [], []
+    for cname, py in structs.items():
+        prints.append(f'printf("{cname} sizeof %zu\\n", sizeof({cname}));')
+        want.append(f"{cname} sizeof {ctypes.sizeof(py)}")
+        for field in (f[0] for f in py._fields_):
+            prints.append(f'printf("{cname} {field} %zu\\n", offsetof({cname}, {field}));')
+            want.append(f"{cname} {field} {getattr(py, field).offset}")
+    code = "#include \"t2h.h\"\n#include <stdio.h>\n#include <stddef.h>\nint main(void) {\n" + "\n".join(prints) + \
+        "\nreturn 0;\n}\n"
     with tempfile.TemporaryDirectory() as td:
         c = os.path.join(td, "s.c")
         open(c, "w").write(code)
         exe = os.path.join(td, "s")
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), c, "-o", exe])
-        got = [int(v) for v in subprocess.check_output([exe]).split()]
-    P = _lib.TapGemmParams
-    W = _lib.ConvWgradParams
-    want = [ctypes.sizeof(P), P.b.offset, P.ntaps.offset, P.d.offset, P.alpha.offset, P.gn_cpg.offset,
-            ctypes.sizeof(W), W.x.offset, W.ntaps.offset, W.dw.offset, W.k_split.offset]
+        got = subprocess.check_output([exe]).decode().splitlines()
     assert got == want
 
 

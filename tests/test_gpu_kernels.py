@@ -236,6 +236,44 @@ def test_fused_groupnorm_statistics_in_conv_epilogue(cuda, C, Cout, H, W):
     assert _rel(s1, torch.stack((o1d.sum((1, 3)), (o1d * o1d).sum((1, 3))), -1)) < 1e-5
 
 
+GN_CONV_CASES = [  # N, H, W, Cin, Cout, terms, residual, nchw
+    (2, 32, 16, 128, 128, 2, True, False), (1, 64, 32, 128, 256, 2, False, False), (2, 16, 8, 256, 256, 2, True, False),
+    (2, 8, 4, 256, 128, 2, False, False), (2, 32, 16, 128, 3, 2, False, True), (2, 32, 16, 128, 128, 1, True, False),
+    (3, 40, 24, 64, 128, 2, False, False), (1, 256, 128, 128, 128, 2, True, False),
+]
+
+
+@pytest.mark.parametrize("case", GN_CONV_CASES, ids=lambda c: "-".join(str(int(v)) for v in c))
+def test_groupnorm_swish_then_conv3x3_matches_fp64(cuda, case):
+    """swish(GroupNorm(x)) -> 3x3 conv (Normalize() + nonlinearity() + Conv2d of ResnetBlock / conv_out,
+    vqgan_arch.py:599-609, :916-918, :1030-1032) as the gn_apply pass and the conv, against fp64 torch; the conv
+    epilogue's GroupNorm sums against fp64 sums of its own output"""
+    from text2human_b200 import ops
+    N, H, W, Ci, Co, terms, residual, nchw = case
+    g = torch.Generator().manual_seed(sum(int(v) for v in case))
+    x = (torch.randn(N, H, W, Ci, generator=g) * 1.5 + 0.3).to(cuda)
+    gamma = (1 + 0.1 * torch.randn(Ci, generator=g)).to(cuda)
+    beta = (0.1 * torch.randn(Ci, generator=g)).to(cuda)
+    w = torch.randn(Co, Ci, 3, 3, generator=g) / (9 * Ci) ** 0.5
+    b = (0.1 * torch.randn(Co, generator=g)).to(cuda)
+    res = torch.randn(N, H, W, Co, generator=g).to(cuda) if residual else None
+    a = ops.group_norm(x, gamma, beta, swish=True, eps=1e-6, terms=terms, stats=ops.norm_stats(x, 32))
+    out = ops.conv3x3(a, ops.pack_conv_weight(w.to(cuda), terms), b, residual=res, nchw_out=nchw,
+                      want_stats=not nchw)
+    if not nchw:
+        out, stats = out
+        if stats is not None:
+            o = out.double().view(N, H * W, 32, Co // 32)
+            assert _rel(stats, torch.stack((o.sum((1, 3)), (o * o).sum((1, 3))), -1)) < 1e-5
+    xr = x.permute(0, 3, 1, 2).double()
+    u = F.group_norm(xr, 32, gamma.double(), beta.double(), eps=1e-6)
+    want = F.conv2d(u * torch.sigmoid(u), w.to(cuda).double(), b.double(), padding=1)
+    if residual:
+        want = want + res.permute(0, 3, 1, 2).double()
+    got = out if nchw else out.permute(0, 3, 1, 2)
+    assert _rel(got, want) < (3e-5 if terms == 2 else 4e-3)
+
+
 @pytest.mark.parametrize("terms", [1, 2])
 @pytest.mark.parametrize("N,H,W,Cin,Cout", [(1, 37, 19, 40, 128), (2, 21, 50, 128, 256), (1, 5, 3, 64, 128),
                                             (3, 33, 17, 72, 72), (1, 512, 256, 8, 128)])

@@ -10,6 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libt2h.so")
 
+ABI_VERSION = 202  # T2H_VERSION of include/t2h.h that the structs below mirror
 MAX_TAPS = 16
 OUT_F32, OUT_PLANES = 0, 1
 BIAS_NONE, BIAS_COL, BIAS_ROW = 0, 1, 2
@@ -42,8 +43,6 @@ class TapGemmParams(C.Structure):
         ("gn_stats", C.c_void_p), ("gn_cpg", C.c_int32), ("a_mn", C.c_int32), ("b_mn", C.c_int32), ("bias_sn", C.c_int64), ("k_split", C.c_int32),
         ("use_tap_w", C.c_int32), ("tap_w", C.c_int32 * MAX_TAPS), ("accumulate", C.c_int32),
         ("k_partials", C.c_int32), ("d_slab", C.c_int64),
-        ("a_f32", C.c_void_p), ("a_gn_stats", C.c_void_p), ("a_gn_gamma", C.c_void_p), ("a_gn_beta", C.c_void_p),
-        ("a_gn_eps", C.c_float), ("a_gn_swish", C.c_int32), ("a_gn_groups", C.c_int32),
         ("nb_sums", C.c_void_p), ("nb_stats", C.c_void_p), ("nb_gamma", C.c_void_p), ("nb_beta", C.c_void_p),
         ("nb_eps", C.c_float), ("nb_act", C.c_int32), ("nb_groups", C.c_int32),
     ]

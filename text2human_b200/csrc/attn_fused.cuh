@@ -278,16 +278,9 @@ extern "C" int t2h_attn_fwd(const void* qkv, int terms, int64_t plane, int64_t l
   P.out = reinterpret_cast<__half*>(out);
   P.out_plane = out_plane;
   P.ld_out = ld_out;
-  {
-    static int dbg = -1;
-    if (dbg < 0) {
-      const char* e = getenv("T2H_DEBUG");
-      dbg = e ? atoi(e) : 0;
-    }
-    P.debug = dbg;
-  }
+  P.debug = debug_bits();
   const int grid = batch * heads * P.qblocks;
-  T2H_CUDA(launch_pdl(attn_fused_kernel, dim3(grid), dim3(kAttnThreads), kAttnSmem, as_stream(stream), 1, tmX, P));
+  T2H_CUDA(launch_pdl(attn_fused_kernel, dim3(grid), dim3(kAttnThreads), kAttnSmem, as_stream(stream), tmX, P));
   T2H_LAUNCH_OK();
   return T2H_OK;
 }

@@ -795,9 +795,9 @@ int t2h_softmax_rows(const float* s, void* out, int64_t rows, int cols, float sc
   const long long plane = rows * cols;
   cudaStream_t st = as_stream(stream);
   if (cols <= 512)
-    T2H_CUDA(launch_pdl(softmax_rows_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, 1, s, o, rows, cols, scale, terms, plane));
+    T2H_CUDA(launch_pdl(softmax_rows_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, s, o, rows, cols, scale, terms, plane));
   else
-    T2H_CUDA(launch_pdl(softmax_rows_kernel<64>, dim3(grid), dim3(warps * 32), 0, st, 1, s, o, rows, cols, scale, terms, plane));
+    T2H_CUDA(launch_pdl(softmax_rows_kernel<64>, dim3(grid), dim3(warps * 32), 0, st, s, o, rows, cols, scale, terms, plane));
   T2H_LAUNCH_OK();
   return T2H_OK;
 }
@@ -813,10 +813,10 @@ int t2h_layernorm(const float* x, const float* gamma, const float* beta, void* o
   const long long plane = rows * c;
   cudaStream_t st = as_stream(stream);
   if (c <= 512)
-    T2H_CUDA(launch_pdl(layernorm_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, 1, x, gamma, beta, o, rows, c, eps, terms, plane,
+    T2H_CUDA(launch_pdl(layernorm_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, x, gamma, beta, o, rows, c, eps, terms, plane,
                         static_cast<const long long*>(nullptr)));
   else
-    T2H_CUDA(launch_pdl(layernorm_kernel<32>, dim3(grid), dim3(warps * 32), 0, st, 1, x, gamma, beta, o, rows, c, eps, terms, plane,
+    T2H_CUDA(launch_pdl(layernorm_kernel<32>, dim3(grid), dim3(warps * 32), 0, st, x, gamma, beta, o, rows, c, eps, terms, plane,
                         static_cast<const long long*>(nullptr)));
   T2H_LAUNCH_OK();
   return T2H_OK;
@@ -839,16 +839,16 @@ int t2h_splitk_reduce_ln(const float* partials, int n_slabs, int64_t slab, const
                                                            reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) % 16 == 0) &&
                        (reinterpret_cast<uintptr_t>(ln_out) % 8 == 0) && (plane % 4 == 0);
   if (aligned && c <= 512)
-    T2H_CUDA(launch_pdl(splitk_reduce_ln_vec_kernel<4>, dim3(grid), dim3(warps * 32), 0, st, 1, partials, n_slabs,
+    T2H_CUDA(launch_pdl(splitk_reduce_ln_vec_kernel<4>, dim3(grid), dim3(warps * 32), 0, st, partials, n_slabs,
                         (long long)slab, bias, residual, x_out, gamma, beta, eps, o, terms, plane, rm, (long long)rows, c));
   else if (aligned)
-    T2H_CUDA(launch_pdl(splitk_reduce_ln_vec_kernel<8>, dim3(grid), dim3(warps * 32), 0, st, 1, partials, n_slabs,
+    T2H_CUDA(launch_pdl(splitk_reduce_ln_vec_kernel<8>, dim3(grid), dim3(warps * 32), 0, st, partials, n_slabs,
                         (long long)slab, bias, residual, x_out, gamma, beta, eps, o, terms, plane, rm, (long long)rows, c));
   else if (c <= 512)
-    T2H_CUDA(launch_pdl(splitk_reduce_ln_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, 1, partials, n_slabs,
+    T2H_CUDA(launch_pdl(splitk_reduce_ln_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, partials, n_slabs,
                         (long long)slab, bias, residual, x_out, gamma, beta, eps, o, terms, plane, rm, (long long)rows, c));
   else
-    T2H_CUDA(launch_pdl(splitk_reduce_ln_kernel<32>, dim3(grid), dim3(warps * 32), 0, st, 1, partials, n_slabs,
+    T2H_CUDA(launch_pdl(splitk_reduce_ln_kernel<32>, dim3(grid), dim3(warps * 32), 0, st, partials, n_slabs,
                         (long long)slab, bias, residual, x_out, gamma, beta, eps, o, terms, plane, rm, (long long)rows, c));
   return T2H_OK;
 }
@@ -858,7 +858,7 @@ int t2h_embed_sum(const int64_t* idx, const int64_t* segm, const int64_t* tex, c
                   int t, int c, t2h_stream_t stream) {
   T2H_CHECK_ARG(idx && segm && tex && tok_emb && pos_emb && segm_emb && tex_emb && x, "embed_sum: null");
   T2H_CHECK_ARG(b > 0 && t > 0 && c > 0 && c % 4 == 0, "embed_sum: bad shape");
-  T2H_CUDA(launch_pdl(embed_sum_kernel, dim3(b * t), dim3(128), 0, as_stream(stream), 1,
+  T2H_CUDA(launch_pdl(embed_sum_kernel, dim3(b * t), dim3(128), 0, as_stream(stream),
                       reinterpret_cast<const long long*>(idx), reinterpret_cast<const long long*>(segm),
                       reinterpret_cast<const long long*>(tex), tok_emb, pos_emb, segm_emb, tex_emb, x, t, c));
   return T2H_OK;
@@ -937,10 +937,10 @@ int t2h_layernorm_scatter(const float* x, const float* gamma, const float* beta,
   const long long* rm = reinterpret_cast<const long long*>(row_map);
   cudaStream_t st = as_stream(stream);
   if (c <= 512)
-    T2H_CUDA(launch_pdl(layernorm_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, 1, x, gamma, beta, o, rows, c, eps,
+    T2H_CUDA(launch_pdl(layernorm_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, x, gamma, beta, o, rows, c, eps,
                         terms, plane, rm));
   else
-    T2H_CUDA(launch_pdl(layernorm_kernel<32>, dim3(grid), dim3(warps * 32), 0, st, 1, x, gamma, beta, o, rows, c, eps,
+    T2H_CUDA(launch_pdl(layernorm_kernel<32>, dim3(grid), dim3(warps * 32), 0, st, x, gamma, beta, o, rows, c, eps,
                         terms, plane, rm));
   return T2H_OK;
 }

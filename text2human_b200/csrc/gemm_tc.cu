@@ -41,8 +41,7 @@ struct TapGemmDev {
   // taps grouped by (dx, img_off): one activation slab per group
   int ngroups, slab_rows;
   int a_slots, b_slots;  // ring depths (A slabs / B tiles)
-  int debug;             // T2H_DEBUG bits (profiling experiments only): 1 skip epilogue work,
-                         // 4 skip TMA loads
+  int debug;             // T2H_DEBUG bits (16: per-launch trace, see g_t2h_dbg)
   int g_dx[T2H_MAX_TAPS], g_ioff[T2H_MAX_TAPS], g_dy0[T2H_MAX_TAPS], g_ntaps[T2H_MAX_TAPS];
   int g_dyrel[T2H_MAX_TAPS][3], g_btap[T2H_MAX_TAPS][3];
   void* d;
@@ -59,13 +58,6 @@ struct TapGemmDev {
   // images, both operands are NHWC planes read MN-major, the output "image" index is the tap whose (dy, dx,
   // img_off) shifts the X patch; accum: the epilogue reduce-adds into D even without split-K
   int wg, accum;
-  // fused GroupNorm(+swish) activation producer (tapgemm_swap_kernel<MBLK, true>): fp32 NHWC source + statistics
-  const float* ax;
-  long long ax_sn, ax_sh, ax_sw;
-  const double* ag_stats;
-  const float *ag_gamma, *ag_beta;
-  float ag_eps;
-  int ag_swish, ag_groups, ag_hw, ag_H, ag_W;
   int partials;  // split-K without reduction: k-slice s of a tile is stored to image slot t.img + s of D
   // norm-backward sums in the swapped kernel's epilogue (see t2h_tapgemm_params.nb_sums): `residual` is x
   double* nb_sums;
@@ -99,17 +91,16 @@ constexpr int kEpiBytes = 4 * kEpiBufBytes;  // 2 output + 2 residual staging ti
 constexpr int kMaxSlots = 8;
 constexpr int kDynSmem = 227 * 1024 - 4096;  // opt-in limit minus ~4 KB of static shared memory
 
-// Tiles are 128 rows (MBLK = 1) by BN <= 128 columns: each consumer warpgroup holds a 64 x BN fp32 accumulator
+// Tiles are 128 rows by BN <= 128 columns: each consumer warpgroup holds a 64 x BN fp32 accumulator
 // (BN / 2 registers per thread) and the [128][BN + 4] staging array (the padding spreads a column's rows over the
 // shared-memory banks) fits beside the operand rings.
-template <int BN, int MBLK>
+template <int BN>
 struct Cfg {
-  static_assert(MBLK == 1 && BN <= 128, "sm_90a tiles are 128 x BN, BN <= 128");
-  // A ring: slabs of (MBLK*TH + 2) x TW positions x 128 bytes (TW <= 16 whenever taps share a slab)
-  static constexpr int kASlot = MBLK * kABlockBytes + 4096;
+  static_assert(BN <= 128, "sm_90a tiles are 128 x BN, BN <= 128");
+  // A ring: slabs of (TH + 2) x TW positions x 128 bytes (TW <= 16 whenever taps share a slab)
+  static constexpr int kASlot = kABlockBytes + 4096;
   static constexpr int kBSlot = BN * 128;
-  static constexpr int kAccCols = MBLK * BN;
-  static constexpr int kStageLd = kAccCols + 4;  // fp32 words per staging row
+  static constexpr int kStageLd = BN + 4;  // fp32 words per staging row
   static constexpr int kStageBytes = 128 * kStageLd * 4;
   static constexpr int kRingBytes = kDynSmem - 1024 - kEpiBytes - kStageBytes;  // A ring + B ring
   static constexpr int kChunk = BN < 32 ? BN : 32;  // columns per staging read in the direct epilogue
@@ -119,7 +110,7 @@ struct TileCoord {
   int img, h0, w0, n0;
 };
 
-__device__ __forceinline__ TileCoord decode_tile(const TapGemmDev& P, int tile, int mblk, int bn) {
+__device__ __forceinline__ TileCoord decode_tile(const TapGemmDev& P, int tile, int bn) {
   TileCoord t;
   int n_tile = tile % P.n_tiles_n;
   int m_tile = tile / P.n_tiles_n;
@@ -133,7 +124,7 @@ __device__ __forceinline__ TileCoord decode_tile(const TapGemmDev& P, int tile, 
   int rem = m_tile - t.img * per_img;
   int ty = rem / P.tiles_w;
   int tx = rem - ty * P.tiles_w;
-  t.h0 = ty * P.TH * mblk;
+  t.h0 = ty * P.TH;
   t.w0 = tx * P.TW;
   t.n0 = n_tile * bn;
   return t;
@@ -183,12 +174,12 @@ __device__ __forceinline__ void gn_accumulate(const float (&v)[32], bool row_ok,
   if (lane < NV) atomicAdd(&gs[idx], vals[0]);
 }
 
-template <int BN, int MBLK>
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
                const __grid_constant__ TapGemmDev P) {
-  using C = Cfg<BN, MBLK>;
+  using C = Cfg<BN>;
   pdl_launch_dependents();  // the next kernel may start its prologue once every CTA of this one is running
   const int NA = P.a_slots, NB = P.b_slots;
   extern __shared__ uint8_t smem_raw[];
@@ -217,7 +208,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if constexpr (BN >= 64) {
     two_groups = P.epi_mode == EPI_TMA_PLANES ||
                  (P.epi_mode == EPI_TMA_F32 && !P.residual && !P.gn_stats && P.act == T2H_ACT_NONE &&
-                  P.bias_mode != T2H_BIAS_ROW && !(P.debug & 1));
+                  P.bias_mode != T2H_BIAS_ROW);
   }
   const int n_epi = two_groups ? 256 : 128;  // threads at the epilogue's named barriers
   __shared__ unsigned long long* trace_s;  // this launch's trace record (CTA 0, T2H_DEBUG bit 16), else null
@@ -268,32 +259,28 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int tile = work % P.total_tiles;
         const int ch0 = (work / P.total_tiles) * P.kper;
         const int ch1 = min(P.kchunks, ch0 + P.kper);
-        const TileCoord t = decode_tile(P, tile, MBLK, BN);
+        const TileCoord t = decode_tile(P, tile, BN);
         const int a_img = P.a_bcast ? 0 : t.img;
         for (int g = 0; g < P.ngroups; ++g) {
           for (int ch = ch0; ch < ch1; ++ch) {
             for (int pl = 0; pl < a_planes; ++pl) {  // hi, then lo
               mbar_wait(&a_empty[sa], pa ^ 1);
-              if (P.debug & 4) {
-                mbar_arrive(&a_full[sa]);
-              } else {
-                if (P.a_mn) {
-                  // [k][row] storage: two boxes of 64 rows x 64 k per 128-row block
-                  mbar_expect_tx(&a_full[sa], kABlockBytes);
-                  int c1 = ch * kBK, c2 = t.h0, c3 = a_img + pl * P.a_term_imgs;
-                  if (P.wg) {  // chunk = one 64-pixel patch of dY: (channel, x, y, image)
-                    const int n = ch / P.wg_ppi, r = ch - n * P.wg_ppi, py = r / P.wg_pw, px = r - py * P.wg_pw;
-                    c1 = px * P.wg_PW; c2 = py * P.wg_PH; c3 = n + pl * P.a_term_imgs;
-                  }
-#pragma unroll
-                  for (int hbox = 0; hbox < 2; ++hbox)
-                    tma_load_4d(&tmA, &a_full[sa], a_ring + sa * C::kASlot + hbox * 8192, t.w0 + 64 * hbox,
-                                c1, c2, c3);
-                } else {
-                  mbar_expect_tx(&a_full[sa], slab_bytes);
-                  tma_load_4d(&tmA, &a_full[sa], a_ring + sa * C::kASlot, ch * kBK, t.w0 + P.g_dx[g],
-                              t.h0 + P.g_dy0[g], a_img + P.g_ioff[g] + pl * P.a_term_imgs);
+              if (P.a_mn) {
+                // [k][row] storage: two boxes of 64 rows x 64 k per 128-row block
+                mbar_expect_tx(&a_full[sa], kABlockBytes);
+                int c1 = ch * kBK, c2 = t.h0, c3 = a_img + pl * P.a_term_imgs;
+                if (P.wg) {  // chunk = one 64-pixel patch of dY: (channel, x, y, image)
+                  const int n = ch / P.wg_ppi, r = ch - n * P.wg_ppi, py = r / P.wg_pw, px = r - py * P.wg_pw;
+                  c1 = px * P.wg_PW; c2 = py * P.wg_PH; c3 = n + pl * P.a_term_imgs;
                 }
+#pragma unroll
+                for (int hbox = 0; hbox < 2; ++hbox)
+                  tma_load_4d(&tmA, &a_full[sa], a_ring + sa * C::kASlot + hbox * 8192, t.w0 + 64 * hbox,
+                              c1, c2, c3);
+              } else {
+                mbar_expect_tx(&a_full[sa], slab_bytes);
+                tma_load_4d(&tmA, &a_full[sa], a_ring + sa * C::kASlot, ch * kBK, t.w0 + P.g_dx[g],
+                            t.h0 + P.g_dy0[g], a_img + P.g_ioff[g] + pl * P.a_term_imgs);
               }
               if (++sa == NA) {
                 sa = 0;
@@ -313,7 +300,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int tile = work % P.total_tiles;
         const int ch0 = (work / P.total_tiles) * P.kper;
         const int ch1 = min(P.kchunks, ch0 + P.kper);
-        const TileCoord t = decode_tile(P, tile, MBLK, BN);
+        const TileCoord t = decode_tile(P, tile, BN);
         const int b_g2 = P.b_batched ? t.img : 0;
         const int b_g = P.b_batched_h ? t.h0 : 0;
         for (int g = 0; g < P.ngroups; ++g) {
@@ -321,24 +308,20 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             for (int tp = 0; tp < P.g_ntaps[g]; ++tp) {
               for (int pl = b_planes - 1; pl >= 0; --pl) {  // lo first, then hi (consumption order)
                 mbar_wait(&b_empty[sb], pb ^ 1);
-                if (P.debug & 4) {
-                  mbar_arrive(&b_full[sb]);
-                } else {
-                  mbar_expect_tx(&b_full[sb], C::kBSlot);
-                  if (P.b_mn) {
-                    // [k][column] storage: one box of 64 columns x 64 k per 64 output columns
-                    int c1 = ch * kBK, c2 = b_g + P.g_btap[g][tp] + pl * P.b_term_g, c3 = b_g2;
-                    if (P.wg) {  // the same patch of X, shifted by this output tile's tap
-                      const int n = ch / P.wg_ppi, r = ch - n * P.wg_ppi, py = r / P.wg_pw, px = r - py * P.wg_pw;
-                      c1 = px * P.wg_PW + P.wg_dx[t.img]; c2 = py * P.wg_PH + P.wg_dy[t.img];
-                      c3 = n + P.wg_ioff[t.img] + pl * P.b_term_g;
-                    }
-                    for (int q = 0; q < BN / 64; ++q)
-                      tma_load_4d(&tmB, &b_full[sb], b_ring + sb * C::kBSlot + q * 8192, t.n0 + 64 * q, c1, c2, c3);
-                  } else {
-                    tma_load_4d(&tmB, &b_full[sb], b_ring + sb * C::kBSlot, ch * kBK, t.n0,
-                                b_g + P.g_btap[g][tp] + pl * P.b_term_g, b_g2);
+                mbar_expect_tx(&b_full[sb], C::kBSlot);
+                if (P.b_mn) {
+                  // [k][column] storage: one box of 64 columns x 64 k per 64 output columns
+                  int c1 = ch * kBK, c2 = b_g + P.g_btap[g][tp] + pl * P.b_term_g, c3 = b_g2;
+                  if (P.wg) {  // the same patch of X, shifted by this output tile's tap
+                    const int n = ch / P.wg_ppi, r = ch - n * P.wg_ppi, py = r / P.wg_pw, px = r - py * P.wg_pw;
+                    c1 = px * P.wg_PW + P.wg_dx[t.img]; c2 = py * P.wg_PH + P.wg_dy[t.img];
+                    c3 = n + P.wg_ioff[t.img] + pl * P.b_term_g;
                   }
+                  for (int q = 0; q < BN / 64; ++q)
+                    tma_load_4d(&tmB, &b_full[sb], b_ring + sb * C::kBSlot + q * 8192, t.n0 + 64 * q, c1, c2, c3);
+                } else {
+                  tma_load_4d(&tmB, &b_full[sb], b_ring + sb * C::kBSlot, ch * kBK, t.n0,
+                              b_g + P.g_btap[g][tp] + pl * P.b_term_g, b_g2);
                 }
                 if (++sb == NB) {
                   sb = 0;
@@ -359,7 +342,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const uint64_t b_desc0 = gmma_desc(smem_u32(b_ring), P.b_mn);
     const uint32_t row16 = (uint32_t)(P.TW * 128) >> 4;  // one slab image row, in 16-byte units
     constexpr uint32_t A16 = C::kASlot >> 4, B16 = C::kBSlot >> 4;
-    const int ngroups = P.ngroups, kchunks = P.kchunks;
+    const int ngroups = P.ngroups;
     int sa = 0, pa = 0, sb = 0, pb = 0;
     // every consumer thread arrives once the warpgroup's MMAs reading the slot have completed (a lane-0 arrival
     // between wgmmas puts them on a divergent path, and ptxas then serialises every MMA)
@@ -371,7 +354,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int th = row / P.TW, tw = row - th * P.TW;
     const bool elected = (threadIdx.x == 128);
     int buf = 0;  // staging buffer toggle (persists across tiles)
-    uint32_t res_par[2] = {0, 0};
+    uint32_t res_par = 0;  // bit b: phase of res_bar[b]
     int tile_par = 0;  // gsum buffer of this tile
 
     for (int work = work0; work < P.total_work; work += work_stride) {
@@ -440,7 +423,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       acc_store_rows(acc, stage, LD, wg, wt);
       named_bar_sync(3, 256);
       if (!epi) continue;
-      const TileCoord t = decode_tile(P, tile, MBLK, BN);
+      const TileCoord t = decode_tile(P, tile, BN);
 
       const bool plain_f32 = two_groups && P.epi_mode == EPI_TMA_F32;
       if (plain_f32) {
@@ -450,22 +433,20 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // general path below
         const int cols_left = P.n_out - t.n0;
         const int nuc = (cols_left >= BN) ? BN / 64 : (cols_left + 63) / 64;
-        const int nunits = MBLK * nuc;
         const bool add_bias = P.bias_mode == T2H_BIAS_COL && ch0 == 0;  // split-K: the first k-slice carries the bias
         if (add_bias) {
           for (int i = threadIdx.x - 128; i < BN; i += 256)
             sbias[i] = (t.n0 + i < P.n_out) ? __ldg(P.bias + t.img * P.bias_sn + t.n0 + i) : 0.f;
         }
         if (trace && elected && work == work0) trace[4] = gtime_ns();
-        for (int u = 0; u < nunits; ++u) {
-          const int mb = u / nuc, cc = u - mb * nuc;
+        for (int cc = 0; cc < nuc; ++cc) {
           const int col0 = t.n0 + cc * 64;
           uint8_t* const o0 = buf ? res_buf : out_buf;
           named_bar_sync(1, n_epi);  // this pair is free (elected waited for the stores issued two units ago)
           {
             const int half = grp;
             uint32_t r[32];
-            stage_ld<32>(stage, LD, row, mb * BN + cc * 64 + half * 32, r);
+            stage_ld<32>(stage, LD, row, cc * 64 + half * 32, r);
             uint8_t* const ob = o0 + half * kEpiBufBytes;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
@@ -487,11 +468,11 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               if (c0 >= P.n_out) break;
               const uint8_t* ob = o0 + half * kEpiBufBytes;
               if (P.partials)  // deterministic split-K: every k-slice owns a slab; a fixed-order pass sums them
-                tma_store_4d(&tmD, ob, c0, t.w0, t.h0 + mb * P.TH, t.img + work / P.total_tiles);
+                tma_store_4d(&tmD, ob, c0, t.w0, t.h0, t.img + work / P.total_tiles);
               else if (P.ksplit > 1 || P.accum)
-                tma_reduce_add_4d(&tmD, ob, c0, t.w0, t.h0 + mb * P.TH, t.img);
+                tma_reduce_add_4d(&tmD, ob, c0, t.w0, t.h0, t.img);
               else
-                tma_store_4d(&tmD, ob, c0, t.w0, t.h0 + mb * P.TH, t.img);
+                tma_store_4d(&tmD, ob, c0, t.w0, t.h0, t.img);
             }
             tma_store_commit();
             tma_store_wait_read<1>();  // the other pair is free again
@@ -501,38 +482,24 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       } else if (P.epi_mode == EPI_TMA_F32) {
         // ---- fp32 NHWC output: 32-column units through swizzled smem + TMA store
         const int cols_left = P.n_out - t.n0;
-        int nuc = (cols_left >= BN) ? BN / 32 : (cols_left + 31) / 32;
-        const int nunits = MBLK * nuc;
+        const int nuc = (cols_left >= BN) ? BN / 32 : (cols_left + 31) / 32;
         const bool has_res = P.residual != nullptr;
-        auto issue_res = [&](int u, int b) {
-          const int mb = u / nuc, cc = u - mb * nuc;
+        auto issue_res = [&](int cc, int b) {
           mbar_expect_tx(&res_bar[b], kEpiBufBytes);
-          tma_load_4d(&tmR, &res_bar[b], res_buf + b * kEpiBufBytes, t.n0 + cc * 32, t.w0,
-                      t.h0 + mb * P.TH, t.img);
+          tma_load_4d(&tmR, &res_bar[b], res_buf + b * kEpiBufBytes, t.n0 + cc * 32, t.w0, t.h0, t.img);
         };
         if (has_res && elected) {
           issue_res(0, buf);
-          if (nunits > 1) issue_res(1, buf ^ 1);
+          if (nuc > 1) issue_res(1, buf ^ 1);
         }
         if (trace && elected && work == work0) trace[4] = gtime_ns();
-        for (int u = 0; u < nunits; ++u) {
-          const int mb = u / nuc, cc = u - mb * nuc;
+        for (int cc = 0; cc < nuc; ++cc) {
           const int col0 = t.n0 + cc * 32;
-          const int h = t.h0 + mb * P.TH + th;
+          const int h = t.h0 + th;
           const int w = t.w0 + tw;
           const bool row_ok = (h < P.H) && (w < P.W);
           uint32_t r[32];
-          stage_ld<32>(stage, LD, row, mb * BN + cc * 32, r);
-          if (P.debug & 1) {
-            if (has_res) {
-              mbar_wait(&res_bar[buf], res_par[buf]);
-              res_par[buf] ^= 1;
-              named_bar_sync(2, 128);
-              if (elected && u + 2 < nunits) issue_res(u + 2, buf);
-            }
-            buf ^= 1;
-            continue;
-          }
+          stage_ld<32>(stage, LD, row, cc * 32, r);
           float v[32];
           const float row_bias =
               (P.bias_mode == T2H_BIAS_ROW && row_ok) ? __ldg(P.bias + h * P.W + w) : 0.f;
@@ -558,8 +525,8 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             for (int i = 0; i < 32; ++i) v[i] = v[i] > 0.f ? v[i] : 0.2f * v[i];
           }
           if (has_res) {
-            mbar_wait(&res_bar[buf], res_par[buf]);
-            res_par[buf] ^= 1;
+            mbar_wait(&res_bar[buf], (res_par >> buf) & 1);
+            res_par ^= 1u << buf;
             const uint8_t* rb = res_buf + buf * kEpiBufBytes;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
@@ -588,13 +555,13 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           named_bar_sync(2, 128);  // staging tile complete; residual tile fully consumed
           if (elected) {
             if (P.partials)  // deterministic split-K: every k-slice owns a slab; a fixed-order pass sums them
-              tma_store_4d(&tmD, ob, col0, t.w0, t.h0 + mb * P.TH, t.img + work / P.total_tiles);
+              tma_store_4d(&tmD, ob, col0, t.w0, t.h0, t.img + work / P.total_tiles);
             else if (P.ksplit > 1 || P.accum)
-              tma_reduce_add_4d(&tmD, ob, col0, t.w0, t.h0 + mb * P.TH, t.img);  // partial sum of a k-slice
+              tma_reduce_add_4d(&tmD, ob, col0, t.w0, t.h0, t.img);  // partial sum of a k-slice
             else
-              tma_store_4d(&tmD, ob, col0, t.w0, t.h0 + mb * P.TH, t.img);
+              tma_store_4d(&tmD, ob, col0, t.w0, t.h0, t.img);
             tma_store_commit();
-            if (has_res && u + 2 < nunits) issue_res(u + 2, buf);
+            if (has_res && cc + 2 < nuc) issue_res(cc + 2, buf);
             tma_store_wait_read<1>();  // the other staging tile is free again
           }
           buf ^= 1;
@@ -616,7 +583,6 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // ---- fp16 plane output: 64-column units, hi and lo tiles staged side by side
         const int cols_left = P.n_out - t.n0;
         const int nuc = (cols_left >= BN) ? BN / 64 : (cols_left + 63) / 64;
-        const int nunits = MBLK * nuc;
         // the tile's column bias goes to shared memory once per tile (broadcast reads below instead of L2 round trips
         // between every accumulator read and the stores); visible after the first named barrier below
         // (single buffer: whoever gets here has passed the previous tile's last named barrier, which every thread
@@ -627,10 +593,9 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             sb[i] = (t.n0 + i < P.n_out) ? __ldg(P.bias + t.img * P.bias_sn + t.n0 + i) : 0.f;
         }
         if (trace && elected && work == work0) trace[4] = gtime_ns();
-        for (int u = 0; u < nunits; ++u) {
-          const int mb = u / nuc, cc = u - mb * nuc;
+        for (int cc = 0; cc < nuc; ++cc) {
           const int col0 = t.n0 + cc * 64;
-          const int h = t.h0 + mb * P.TH + th;
+          const int h = t.h0 + th;
           const int w = t.w0 + tw;
           const bool row_ok = (h < P.H) && (w < P.W);
           const float row_bias =
@@ -643,7 +608,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
           for (int half = two_groups ? grp : 0; half < (two_groups ? grp + 1 : 2); ++half) {
             uint32_t r[32];
-            stage_ld<32>(stage, LD, row, mb * BN + cc * 64 + half * 32, r);
+            stage_ld<32>(stage, LD, row, cc * 64 + half * 32, r);
             float v[32];
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]) * P.alpha + row_bias;
@@ -678,9 +643,9 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           fence_proxy_async_smem();
           named_bar_sync(2, n_epi);
           if (elected) {
-            tma_store_4d(&tmD, ohi, col0, t.w0, t.h0 + mb * P.TH, t.img);
+            tma_store_4d(&tmD, ohi, col0, t.w0, t.h0, t.img);
             if (P.d_terms == 2)
-              tma_store_4d(&tmD, olo, col0, t.w0, t.h0 + mb * P.TH, t.img + P.d_term_imgs);
+              tma_store_4d(&tmD, olo, col0, t.w0, t.h0, t.img + P.d_term_imgs);
             tma_store_commit();
             tma_store_wait_read<1>();  // the other pair of staging tiles is free again
           }
@@ -690,60 +655,57 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // ---- direct path: strided / tiny outputs (NCHW conv_out, n_out < 32, unaligned)
         constexpr int CH = C::kChunk;
         if (trace && elected && work == work0) trace[4] = gtime_ns();
+        const int h = t.h0 + th;
+        const int w = t.w0 + tw;
+        const bool row_ok = (h < P.H) && (w < P.W);
+        const long long off = (long long)t.img * P.d_sn + (long long)h * P.d_sh + (long long)w * P.d_sw;
+        const float row_bias = (P.bias_mode == T2H_BIAS_ROW && row_ok) ? P.bias[h * P.W + w] : 0.f;
 #pragma unroll 1
-        for (int mb = 0; mb < MBLK; ++mb) {
-          const int h = t.h0 + mb * P.TH + th;
-          const int w = t.w0 + tw;
-          const bool row_ok = (h < P.H) && (w < P.W);
-          const long long off = (long long)t.img * P.d_sn + (long long)h * P.d_sh + (long long)w * P.d_sw;
-          const float row_bias = (P.bias_mode == T2H_BIAS_ROW && row_ok) ? P.bias[h * P.W + w] : 0.f;
-#pragma unroll 1
-          for (int cc = 0; cc < BN / CH; ++cc) {
-            const int col0 = t.n0 + cc * CH;
-            if (col0 >= P.n_out) break;  // warp-uniform
-            uint32_t r[32];
-            stage_ld<CH>(stage, LD, row, mb * BN + cc * CH, r);
-            if (!row_ok) continue;
-            float v[CH];
+        for (int cc = 0; cc < BN / CH; ++cc) {
+          const int col0 = t.n0 + cc * CH;
+          if (col0 >= P.n_out) break;  // warp-uniform
+          uint32_t r[32];
+          stage_ld<CH>(stage, LD, row, cc * CH, r);
+          if (!row_ok) continue;
+          float v[CH];
 #pragma unroll
-            for (int i = 0; i < CH; ++i) v[i] = __uint_as_float(r[i]) * P.alpha + row_bias;
-            if (P.bias_mode == T2H_BIAS_COL) {
+          for (int i = 0; i < CH; ++i) v[i] = __uint_as_float(r[i]) * P.alpha + row_bias;
+          if (P.bias_mode == T2H_BIAS_COL) {
 #pragma unroll
-              for (int i = 0; i < CH; ++i)
-                if (col0 + i < P.n_out) v[i] += __ldg(P.bias + t.img * P.bias_sn + col0 + i);
-            }
-            if (P.act == T2H_ACT_GELU) {
+            for (int i = 0; i < CH; ++i)
+              if (col0 + i < P.n_out) v[i] += __ldg(P.bias + t.img * P.bias_sn + col0 + i);
+          }
+          if (P.act == T2H_ACT_GELU) {
 #pragma unroll
-              for (int i = 0; i < CH; ++i) v[i] = gelu_erf(v[i]);
-            } else if (P.act == T2H_ACT_RELU) {
+            for (int i = 0; i < CH; ++i) v[i] = gelu_erf(v[i]);
+          } else if (P.act == T2H_ACT_RELU) {
 #pragma unroll
-              for (int i = 0; i < CH; ++i) v[i] = fmaxf(v[i], 0.f);
-            } else if (P.act == T2H_ACT_LRELU) {
+            for (int i = 0; i < CH; ++i) v[i] = fmaxf(v[i], 0.f);
+          } else if (P.act == T2H_ACT_LRELU) {
 #pragma unroll
-              for (int i = 0; i < CH; ++i) v[i] = v[i] > 0.f ? v[i] : 0.2f * v[i];
-            }
-            if (P.d_mode == T2H_OUT_F32) {
-              float* dst = reinterpret_cast<float*>(P.d);
+            for (int i = 0; i < CH; ++i) v[i] = v[i] > 0.f ? v[i] : 0.2f * v[i];
+          }
+          if (P.d_mode == T2H_OUT_F32) {
+            float* dst = reinterpret_cast<float*>(P.d);
 #pragma unroll
-              for (int i = 0; i < CH; ++i) {
-                if (col0 + i < P.n_out) {
-                  const long long o = off + (long long)(col0 + i) * P.d_sc;
-                  float val = v[i];
-                  if (P.residual) val += P.residual[o];
-                  dst[o] = val;
-                }
+            for (int i = 0; i < CH; ++i) {
+              if (col0 + i < P.n_out) {
+                const long long o = off + (long long)(col0 + i) * P.d_sc;
+                float val = v[i];
+                if (P.residual) val += P.residual[o];
+                dst[o] = val;
               }
-            } else {
-              __half* dst = reinterpret_cast<__half*>(P.d);
+            }
+          } else {
+            __half* dst = reinterpret_cast<__half*>(P.d);
 #pragma unroll
-              for (int i = 0; i < CH; ++i) {
-                if (col0 + i < P.n_out) {
-                  const long long o = off + (long long)(col0 + i) * P.d_sc;
-                  __half hi, lo;
-                  split_f16(v[i], hi, lo);
-                  dst[o] = hi;
-                  if (P.d_terms == 2) dst[P.d_plane + o] = lo;
-                }
+            for (int i = 0; i < CH; ++i) {
+              if (col0 + i < P.n_out) {
+                const long long o = off + (long long)(col0 + i) * P.d_sc;
+                __half hi, lo;
+                split_f16(v[i], hi, lo);
+                dst[o] = hi;
+                if (P.d_terms == 2) dst[P.d_plane + o] = lo;
               }
             }
           }
@@ -814,71 +776,52 @@ static int make_tmap(CUtensorMap* tm, const void* base, int elem_bytes, int rank
   return T2H_OK;
 }
 
-template <int BN, int MBLK>
+template <int BN>
 static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
                   const CUtensorMap& tmR, const TapGemmDev& P, cudaStream_t stream) {
-  using C = Cfg<BN, MBLK>;
+  using C = Cfg<BN>;
   static bool configured[64] = {};
   int dev = 0;
   T2H_CUDA(cudaGetDevice(&dev));
   if (!configured[dev & 63]) {  // per device: the attribute lives in the device's copy of the function
-    T2H_CUDA(cudaFuncSetAttribute(tapgemm_kernel<BN, MBLK>,
+    T2H_CUDA(cudaFuncSetAttribute(tapgemm_kernel<BN>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, kDynSmem));
     configured[dev & 63] = true;
   }
   // ring depths: enough bytes in flight to cover the TMA round trip at the tile's consumption rate.
   // With the 3-product split both (hi, lo) slabs of a (group, chunk) are live at once.
   TapGemmDev Q = P;
-  {
-    static int dbg = -1;
-    if (dbg < 0) {
-      const char* e = getenv("T2H_DEBUG");
-      dbg = e ? atoi(e) : 0;
-    }
-    Q.debug = dbg;
-  }
+  Q.debug = debug_bits();
   Q.a_slots = 3;
   int nb = (C::kRingBytes - Q.a_slots * C::kASlot) / C::kBSlot;
   Q.b_slots = nb > kMaxSlots ? kMaxSlots : nb;
   if (Q.b_slots < 2) return fail(T2H_EINVAL, "tapgemm: shared-memory rings do not fit");
   int grid = P.total_work < num_sms() ? P.total_work : num_sms();
   // the full dynamic allocation keeps it to one CTA per SM
-  T2H_CUDA(launch_pdl(tapgemm_kernel<BN, MBLK>, dim3(grid), dim3(kThreads), kDynSmem, stream, 1, tmA,
-                      tmB, tmD, tmR, Q));
+  T2H_CUDA(launch_pdl(tapgemm_kernel<BN>, dim3(grid), dim3(kThreads), kDynSmem, stream, tmA, tmB, tmD, tmR, Q));
   return T2H_OK;
 }
 
-template <int MBLK, bool FUSE>
 static int launch_swap(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
                        const CUtensorMap& tmR, const TapGemmDev& P, cudaStream_t stream) {
-  using C = Cfg<128, MBLK>;
+  using C = Cfg<128>;
   static bool configured[64] = {};
   int dev = 0;
   T2H_CUDA(cudaGetDevice(&dev));
   if (!configured[dev & 63]) {
-    T2H_CUDA(cudaFuncSetAttribute(tapgemm_swap_kernel<MBLK, FUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  kDynSmem));
+    T2H_CUDA(cudaFuncSetAttribute(tapgemm_swap_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDynSmem));
     configured[dev & 63] = true;
   }
   TapGemmDev Q = P;
-  {
-    static int dbg = -1;
-    if (dbg < 0) {
-      const char* e = getenv("T2H_DEBUG");
-      dbg = e ? atoi(e) : 0;
-    }
-    Q.debug = dbg;
-  }
   // ring depths from what the register epilogue leaves of the shared memory: 4 A slabs load the next chunk's hi and
   // lo slabs during the whole current chunk, the rest holds weight tiles (4: two taps of the 3-product order ahead).
-  // The kernel's ring invariant needs a_slots >= 3 and b_slots >= 2.
+  // The kernel's ring invariant needs a_slots >= 2 and b_slots >= 2.
   Q.a_slots = 4;
   int nb = (kSwapRingBytes - Q.a_slots * C::kASlot) / C::kBSlot;
   Q.b_slots = nb > kMaxSlots ? kMaxSlots : nb;
   if (Q.b_slots < 2) return fail(T2H_EINVAL, "tapgemm: shared-memory rings do not fit");
   int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
-  T2H_CUDA(launch_pdl(tapgemm_swap_kernel<MBLK, FUSE>, dim3(grid), dim3(kSwapThreads), kDynSmem, stream, 1, tmA, tmB,
-                      tmD, tmR, Q));
+  T2H_CUDA(launch_pdl(tapgemm_swap_kernel, dim3(grid), dim3(kSwapThreads), kDynSmem, stream, tmA, tmB, tmD, tmR, Q));
   return T2H_OK;
 }
 
@@ -900,13 +843,13 @@ extern "C" int t2h_debug_read(long long* out, int n) {
 }
 
 extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
-  T2H_CHECK_ARG(p && (p->a || p->a_f32) && p->b && p->d, "tapgemm: null operand");
+  T2H_CHECK_ARG(p && p->a && p->b && p->d, "tapgemm: null operand");
   T2H_CHECK_ARG(p->n_img > 0 && p->H > 0 && p->W > 0 && p->C > 0 && p->n_out > 0,
                 "tapgemm: empty problem (n_img=%d H=%d W=%d C=%d n_out=%d)", p->n_img, p->H, p->W, p->C,
                 p->n_out);
   T2H_CHECK_ARG(p->ntaps >= 1 && p->ntaps <= T2H_MAX_TAPS, "tapgemm: ntaps=%d", p->ntaps);
   T2H_CHECK_ARG(p->nterms == 1 || p->nterms == 3, "tapgemm: nterms must be 1 or 3 (got %d)", p->nterms);
-  T2H_CHECK_ARG(p->nterms == 1 || ((p->a_terms == 2 || p->a_f32) && p->b_terms == 2),
+  T2H_CHECK_ARG(p->nterms == 1 || (p->a_terms == 2 && p->b_terms == 2),
                 "tapgemm: nterms=3 needs hi/lo planes on both operands");
   T2H_CHECK_ARG(p->d_mode == T2H_OUT_F32 || p->d_mode == T2H_OUT_PLANES, "tapgemm: d_mode=%d", p->d_mode);
   T2H_CHECK_ARG(p->d_mode == T2H_OUT_F32 || p->d_terms == 1 || p->d_terms == 2, "tapgemm: d_terms=%d",
@@ -958,27 +901,6 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
                            p->d_sc != 1 && p->bias_mode != T2H_BIAS_ROW && !p->a_bcast && !p->b_batched &&
                            !p->b_batched_h && !p->residual && !p->gn_stats && p->act == T2H_ACT_NONE;
   if (swap_direct) swap = true;
-  {
-    static int no_swap = -1;
-    if (no_swap < 0) {
-      const char* e = getenv("T2H_NO_SWAP");
-      no_swap = e ? atoi(e) : 0;
-    }
-    if (no_swap) swap = false;
-  }
-  if (p->a_f32) {
-    // fused GroupNorm(+swish) producer: only in the swapped kernel, whole 64-channel chunks, table of <= 256 channels
-    bool ok = swap && p->C % 64 == 0 && p->C <= 256 && p->a_gn_stats && p->a_gn_gamma && p->a_gn_beta &&
-              p->a_gn_groups > 0 && p->C % p->a_gn_groups == 0 && !p->a_bcast &&
-              reinterpret_cast<uintptr_t>(p->a_f32) % 16 == 0 && p->a_sw % 4 == 0 && p->a_sh % 4 == 0 && p->a_sn % 4 == 0;
-    for (int i = 0; i < p->ntaps; ++i) ok = ok && p->tap_img_off[i] == 0;
-    T2H_CHECK_ARG(ok, "tapgemm: the fused GroupNorm producer needs a swapped-kernel conv (Cout %% 128 == 0 or a strided "
-                      "small-Cout output), C %% 64 == 0, C <= 256 and aligned fp32 NHWC input (C=%d n_out=%d)", p->C, p->n_out);
-    P.ax = p->a_f32; P.ax_sn = p->a_sn; P.ax_sh = p->a_sh; P.ax_sw = p->a_sw;
-    P.ag_stats = p->a_gn_stats; P.ag_gamma = p->a_gn_gamma; P.ag_beta = p->a_gn_beta; P.ag_eps = p->a_gn_eps;
-    P.ag_swish = p->a_gn_swish; P.ag_groups = p->a_gn_groups; P.ag_hw = p->a_H * p->a_W;
-    P.ag_H = p->a_H; P.ag_W = p->a_W;
-  }
   if (p->a_mn || p->b_mn) {
     T2H_CHECK_ARG(rows_mode && p->ntaps == 1 && p->tap_dx[0] == 0 && p->tap_dy[0] == 0,
                   "tapgemm: a_mn / b_mn operands need a row GEMM (H == 1 or tile_rows) with one tap");
@@ -988,7 +910,6 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
   while (BN < p->n_out && BN < 128) BN <<= 1;
   if (p->b_mn && BN < 64) BN = 64;  // an MN-major B tile is made of whole 64-column boxes
   if (swap) BN = 128;
-  const int MBLK = 1;
   P.TW = TW; P.TH = TH;
   // ---- tap groups: taps with the same (dx, img_off) share one activation slab when a vertical
   // shift of the slab view stays 1024-byte aligned (TW*128 bytes per image row, TW >= 8)
@@ -1024,10 +945,10 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
     for (int g = P.ngroups; g < T2H_MAX_TAPS; ++g) {
       P.g_dx[g] = P.g_ioff[g] = P.g_dy0[g] = P.g_ntaps[g] = 0;
     }
-    P.slab_rows = MBLK * TH + extra;
+    P.slab_rows = TH + extra;
   }
   P.tiles_w = ceil_div(p->W, TW);
-  P.tiles_h = ceil_div(p->H, TH * MBLK);
+  P.tiles_h = ceil_div(p->H, TH);
   P.n_tiles_n = ceil_div(p->n_out, BN);
   long long total = (long long)p->n_img * P.tiles_w * P.tiles_h * P.n_tiles_n;
   T2H_CHECK_ARG(total < (1LL << 31), "tapgemm: too many tiles");
@@ -1054,7 +975,7 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
   if (swap) P.epi_mode = swap_direct ? EPI_DIRECT : EPI_TMA_F32;
   if (p->nb_sums) {
     T2H_CHECK_ARG(swap && !swap_direct && p->residual && p->nb_stats && p->nb_gamma && p->nb_beta && !p->gn_stats &&
-                      !p->a_f32 && p->act == T2H_ACT_NONE && p->nb_act >= 0 && p->nb_act <= 2 && p->nb_groups > 0 &&
+                      p->act == T2H_ACT_NONE && p->nb_act >= 0 && p->nb_act <= 2 && p->nb_groups > 0 &&
                       p->n_out % p->nb_groups == 0 && p->k_split <= 1 && !p->accumulate && !p->k_partials,
                   "tapgemm: nb_sums needs a swapped-kernel conv (n_out %% 128 == 0, fp32 NHWC output), x in `residual`, "
                   "statistics / gamma / beta, and no other epilogue work");
@@ -1096,7 +1017,7 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
 
   // ---- tensor maps
   CUtensorMap tmA, tmB, tmD, tmR;
-  if (!p->a_f32) {
+  {
     uint64_t dims[4] = {(uint64_t)p->C, (uint64_t)p->a_W, (uint64_t)p->a_H, (uint64_t)p->a_imgs};
     uint64_t str[4] = {1, (uint64_t)p->a_sw, (uint64_t)p->a_sh, (uint64_t)p->a_sn};
     uint32_t box[4] = {(uint32_t)kBK, (uint32_t)TW, (uint32_t)P.slab_rows, 1};
@@ -1120,7 +1041,6 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
     int rc = make_tmap(&tmB, p->b, 2, 4, dims, str, box, "tapgemm B");
     if (rc) return rc;
   }
-  if (p->a_f32) tmA = tmB;  // unused by the fused-producer kernel
   tmD = tmA;
   tmR = tmA;
   if (P.epi_mode != EPI_DIRECT) {
@@ -1157,13 +1077,12 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
   }
 
   cudaStream_t s = as_stream(stream);
-  if (swap && p->a_f32) return launch_swap<1, true>(tmA, tmB, tmD, tmR, P, s);
-  if (swap) return launch_swap<1, false>(tmA, tmB, tmD, tmR, P, s);
+  if (swap) return launch_swap(tmA, tmB, tmD, tmR, P, s);
   switch (BN) {
-    case 16: return launch<16, 1>(tmA, tmB, tmD, tmR, P, s);
-    case 32: return launch<32, 1>(tmA, tmB, tmD, tmR, P, s);
-    case 64: return launch<64, 1>(tmA, tmB, tmD, tmR, P, s);
-    default: return launch<128, 1>(tmA, tmB, tmD, tmR, P, s);
+    case 16: return launch<16>(tmA, tmB, tmD, tmR, P, s);
+    case 32: return launch<32>(tmA, tmB, tmD, tmR, P, s);
+    case 64: return launch<64>(tmA, tmB, tmD, tmR, P, s);
+    default: return launch<128>(tmA, tmB, tmD, tmR, P, s);
   }
 }
 
@@ -1243,7 +1162,7 @@ extern "C" int t2h_conv_wgrad(const t2h_conv_wgrad_params* p, t2h_stream_t strea
   }
   tmR = tmA;
   cudaStream_t s = as_stream(stream);
-  return BN == 64 ? launch<64, 1>(tmA, tmB, tmD, tmR, P, s) : launch<128, 1>(tmA, tmB, tmD, tmR, P, s);
+  return BN == 64 ? launch<64>(tmA, tmB, tmD, tmR, P, s) : launch<128>(tmA, tmB, tmD, tmR, P, s);
 }
 
 #include "attn_fused.cuh"

@@ -21,21 +21,17 @@
 namespace t2h {
 
 constexpr int kSwapThreads = 384;  // 4 producer warps + 8 consumer warps (two warpgroups of 64 output channels)
-constexpr int kFuseThreads = 96;   // FUSE: warps 0-2 build the activation slabs
 constexpr int kSwapBox = 32 * 16 * 4;         // one TMA box of the epilogue: 32 pixels x 16 fp32 channels
 constexpr int kSwapWarpBuf = 4 * kSwapBox;    // a consumer warp's 128 pixels: residual in, output out, in place
 static_assert(8 * kSwapWarpBuf == kEpiBytes, "epilogue boxes");
 constexpr int kSwapRingBytes = kDynSmem - 1024 - kEpiBytes;  // A ring + B ring
 // Register split (setmaxnreg): the producer warpgroup only issues TMA and waits on barriers; the consumers hold a
 // 64-register accumulator plus the epilogue's values.  The split redistributes what the CTA was launched with, 384
-// threads x 168 registers (the __launch_bounds__ ceiling): 128 x 40 + 256 x 232.  The fused GroupNorm producer does
-// real arithmetic in warps 0-2 and keeps more: 128 x 104 + 256 x 200.
-template <bool FUSE>
-struct SwapRegs {
-  static constexpr int kProducer = FUSE ? 104 : 40;
-  static constexpr int kConsumer = FUSE ? 200 : 232;
-  static_assert(128 * kProducer + 256 * kConsumer <= kSwapThreads * 168, "register split exceeds the CTA's registers");
-};
+// threads x 168 registers (the __launch_bounds__ ceiling): 128 x 40 + 256 x 232.
+constexpr int kSwapProducerRegs = 40;
+constexpr int kSwapConsumerRegs = 232;
+static_assert(128 * kSwapProducerRegs + 256 * kSwapConsumerRegs <= kSwapThreads * 168,
+              "register split exceeds the CTA's registers");
 
 // byte offset of fp32 channel c (0..15) of pixel i (0..31) in a [32][16] box TMA wrote with the 64-byte swizzle
 // (address bits [4,6) ^= bits [7,9))
@@ -69,27 +65,17 @@ __device__ __forceinline__ void nb_flush(const TapGemmDev& P, int img, int c, in
   }
 }
 
-// FUSE = true: the activation operand is NOT read as fp16 planes by TMA.  The kernel takes the fp32 NHWC tensor the
-// previous conv wrote plus its GroupNorm statistics, and three producer warps (0-2) build the swizzled hi / lo slabs
-// the MMAs read themselves: 128-bit loads -> (x - mean) * rstd * gamma + beta ->
-// swish -> fp16 split -> st.shared in the 128-byte-swizzle image a TMA box would have produced.  This is
-// Normalize() + nonlinearity() (vqgan_arch.py:510-517) folded into the consuming conv: the gn_apply pass and its
-// 8 bytes per element of HBM traffic disappear.  Same arithmetic, same order as gn_apply_kernel -> identical slabs.
-//
 // Ring invariant: no group waits on a slot whose release is deferred behind it.  When a group's operands are waited
 // for, every slot whose last reader is two or more groups back has been released.  Each group reads one B tile and
 // the B index advances by at most one per group, so the tile a group needs reuses a slot released two groups back
 // whenever b_slots >= 2.  A slabs (3-product order hi.lo, hi.hi, lo.hi per tap): the next chunk's hi slab reuses the
 // slot of the current chunk's hi slab (last read by the hi.hi group before the chunk's final group) when
-// a_slots >= 2; the FUSE producer claims a chunk's hi and lo slots together before it marks either full, so it also
-// needs the current chunk's lo slot's predecessor free: a_slots >= 3.  1-product: one slab per chunk, a_slots >= 2.
-template <int MBLK, bool FUSE>
+// a_slots >= 2.  1-product: one slab per chunk, a_slots >= 2.
 __global__ void __launch_bounds__(kSwapThreads, 1)
 tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
                     const __grid_constant__ TapGemmDev P) {
-  using C = Cfg<128, MBLK>;
-  static_assert(MBLK == 1, "the register epilogue covers 128-pixel tiles");
+  using C = Cfg<128>;
   pdl_launch_dependents();  // the next kernel may start its prologue once every CTA of this one is running
   const int NA = P.a_slots, NB = P.b_slots;
   extern __shared__ uint8_t smem_raw[];
@@ -104,13 +90,12 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   __shared__ __align__(8) uint64_t b_full[kMaxSlots];
   __shared__ __align__(8) uint64_t b_empty[kMaxSlots];
   __shared__ __align__(8) uint64_t res_bar[8];
-  __shared__ float gn_tab[FUSE ? 512 : 1];  // FUSE: per-channel scale | shift of the current image (C <= 256)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   if (warp == 0 && lane == 0) {
-    if (!FUSE) tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (P.epi_mode != EPI_DIRECT) tma_prefetch_desc(&tmD);
     if (P.residual) tma_prefetch_desc(&tmR);
@@ -145,106 +130,20 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (warp < 4) {
     // (each role's setmaxnreg sits inside its branch: ptxas ignores a reallocation that code needing more registers
     // can follow)
-    setmaxnreg_dec<SwapRegs<FUSE>::kProducer>();
-    if (FUSE && warp < 3) {
-      // ---------------------------------------------- activation slab producers: GroupNorm + swish + fp16 split
-      const int pt = threadIdx.x;  // 0..kFuseThreads-1
-      float* s_scale = gn_tab;
-      float* s_shift = gn_tab + 256;
-      const int tw_shift = 31 - __clz(P.TW);
-      const int R = P.slab_rows * P.TW;  // pixels of one slab
-      const int units = R * 8;           // 8 channels (one 16-byte smem chunk) each
-      const int cpg = P.C / P.ag_groups;
-      const double cnt = (double)P.ag_hw * cpg;
-      int cur_img = -1;
-      int sa = 0, pa = 0;
-      for (int tile = tile_first; tile < tile_end; tile += tile_step) {
-        const TileCoord t = decode_tile(P, tile, MBLK, 128);
-        if (t.img != cur_img) {
-          named_bar_sync(3, kFuseThreads);  // nobody still reads the previous image's table
-          for (int c = pt; c < P.C; c += kFuseThreads) {
-            const int g = c / cpg;
-            const double su = P.ag_stats[((long long)t.img * P.ag_groups + g) * 2 + 0];
-            const double sq = P.ag_stats[((long long)t.img * P.ag_groups + g) * 2 + 1];
-            const double mean = su / cnt;
-            double var = sq / cnt - mean * mean;
-            if (var < 0) var = 0;
-            const float rstd = (float)(1.0 / sqrt(var + (double)P.ag_eps));
-            const float ga = P.ag_gamma[c] * rstd;
-            s_scale[c] = ga;
-            s_shift[c] = P.ag_beta[c] - (float)mean * ga;
-          }
-          named_bar_sync(3, kFuseThreads);
-          cur_img = t.img;
-        }
-        const float* ximg = P.ax + (long long)t.img * P.ax_sn;
-        for (int g = 0; g < P.ngroups; ++g) {
-          const int h_base = t.h0 + P.g_dy0[g], w_base = t.w0 + P.g_dx[g];
-          for (int ch = 0; ch < P.kchunks; ++ch) {
-            const int s_hi = sa;
-            mbar_wait(&a_empty[sa], pa ^ 1);
-            if (++sa == NA) { sa = 0; pa ^= 1; }
-            int s_lo = -1;
-            if (a_planes == 2) {
-              s_lo = sa;
-              mbar_wait(&a_empty[sa], pa ^ 1);
-              if (++sa == NA) { sa = 0; pa ^= 1; }
-            }
-            uint8_t* hi_base = a_ring + s_hi * C::kASlot;
-            uint8_t* lo_base = a_ring + (s_lo >= 0 ? s_lo : s_hi) * C::kASlot;
-            const int c0 = ch * kBK;
-  #pragma unroll 4
-            for (int u = pt; u < units; u += kFuseThreads) {
-              const int r = u >> 3, j = u & 7;
-              const int h = h_base + (r >> tw_shift), w = w_base + (r & (P.TW - 1));
-              const bool ok = (h >= 0) && (h < P.ag_H) && (w >= 0) && (w < P.ag_W);
-              const float* src = ximg + (long long)h * P.ax_sh + (long long)w * P.ax_sw + c0 + j * 8;
-              float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
-              if (ok) {
-                v0 = __ldg(reinterpret_cast<const float4*>(src));
-                v1 = __ldg(reinterpret_cast<const float4*>(src) + 1);
-              }
-              const float f[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-              __align__(16) __half hh[8];
-              __align__(16) __half ll[8];
-  #pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                float y = 0.f;
-                if (ok) {   // conv zero padding applies to the NORMALISED activation: outside pixels stay 0
-                  y = f[e] * s_scale[c0 + j * 8 + e] + s_shift[c0 + j * 8 + e];
-                  if (P.ag_swish) y = y / (1.0f + __expf(-y));
-                }
-                split_f16(y, hh[e], ll[e]);
-              }
-              *reinterpret_cast<uint4*>(hi_base + swz(r, j)) = *reinterpret_cast<const uint4*>(hh);
-              if (s_lo >= 0) *reinterpret_cast<uint4*>(lo_base + swz(r, j)) = *reinterpret_cast<const uint4*>(ll);
-            }
-            fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core's async proxy
-            named_bar_sync(3, kFuseThreads);
-            if (pt == 0) {
-              mbar_arrive(&a_full[s_hi]);
-              if (s_lo >= 0) mbar_arrive(&a_full[s_lo]);
-            }
-          }
-        }
-      }
-    } else if (!FUSE && warp == 0) {
+    setmaxnreg_dec<kSwapProducerRegs>();
+    if (warp == 0) {
       // ---------------------------------------------- activation slab producer
       if (lane == 0) {
         int sa = 0, pa = 0;
         for (int tile = tile_first; tile < tile_end; tile += tile_step) {
-          const TileCoord t = decode_tile(P, tile, MBLK, 128);
+          const TileCoord t = decode_tile(P, tile, 128);
           for (int g = 0; g < P.ngroups; ++g)
             for (int ch = 0; ch < P.kchunks; ++ch)
               for (int pl = 0; pl < a_planes; ++pl) {
                 mbar_wait(&a_empty[sa], pa ^ 1);
-                if (P.debug & 4) {
-                  mbar_arrive(&a_full[sa]);
-                } else {
-                  mbar_expect_tx(&a_full[sa], slab_bytes);
-                  tma_load_4d(&tmA, &a_full[sa], a_ring + sa * C::kASlot, ch * kBK, t.w0 + P.g_dx[g],
-                              t.h0 + P.g_dy0[g], t.img + P.g_ioff[g] + pl * P.a_term_imgs);
-                }
+                mbar_expect_tx(&a_full[sa], slab_bytes);
+                tma_load_4d(&tmA, &a_full[sa], a_ring + sa * C::kASlot, ch * kBK, t.w0 + P.g_dx[g],
+                            t.h0 + P.g_dy0[g], t.img + P.g_ioff[g] + pl * P.a_term_imgs);
                 if (++sa == NA) {
                   sa = 0;
                   pa ^= 1;
@@ -257,19 +156,15 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       if (lane == 0) {
         int sb = 0, pb = 0;
         for (int tile = tile_first; tile < tile_end; tile += tile_step) {
-          const TileCoord t = decode_tile(P, tile, MBLK, 128);
+          const TileCoord t = decode_tile(P, tile, 128);
           for (int g = 0; g < P.ngroups; ++g)
             for (int ch = 0; ch < P.kchunks; ++ch)
               for (int tp = 0; tp < P.g_ntaps[g]; ++tp)
                 for (int pl = a_planes - 1; pl >= 0; --pl) {  // lo first, then hi
                   mbar_wait(&b_empty[sb], pb ^ 1);
-                  if (P.debug & 4) {
-                    mbar_arrive(&b_full[sb]);
-                  } else {
-                    mbar_expect_tx(&b_full[sb], C::kBSlot);
-                    tma_load_4d(&tmB, &b_full[sb], b_ring + sb * C::kBSlot, ch * kBK, t.n0,
-                                P.g_btap[g][tp] + pl * P.b_term_g, 0);
-                  }
+                  mbar_expect_tx(&b_full[sb], C::kBSlot);
+                  tma_load_4d(&tmB, &b_full[sb], b_ring + sb * C::kBSlot, ch * kBK, t.n0,
+                              P.g_btap[g][tp] + pl * P.b_term_g, 0);
                   if (++sb == NB) {
                     sb = 0;
                     pb ^= 1;
@@ -280,7 +175,7 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     }
   } else {
     // ---------------------------------------------- consumers: D^T[cout, pixel] += W * slab^T, then the epilogue
-    setmaxnreg_inc<SwapRegs<FUSE>::kConsumer>();
+    setmaxnreg_inc<kSwapConsumerRegs>();
     const int wg = (warp - 4) >> 2;  // output channels 64 wg .. 64 wg + 63 of the tile
     const uint32_t row16 = (uint32_t)(P.TW * 128) >> 4;  // one slab image row, in 16-byte units
     const uint64_t x_desc0 = gmma_desc(smem_u32(a_ring));
@@ -298,8 +193,8 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     uint32_t res_par = 0;
     const int cpg = P.gn_cpg;
     const int red = 4 * (cpg < 8 ? cpg : 8);  // lanes holding one GroupNorm group's (channel, pixel) partial sums
-    // norm-backward sums: the "residual" tile is x and is not added (never with the fused producer: the host rejects it)
-    const bool nb = !FUSE && P.nb_sums != nullptr;
+    // norm-backward sums: the "residual" tile is x and is not added
+    const bool nb = P.nb_sums != nullptr;
     // per thread: channel c (index 0) and c + 8 (index 1); the sums run on across consecutive tiles of the same
     // (image, channel block) and are flushed when that changes
     float nb_mean[2] = {0.f, 0.f}, nb_rstd[2] = {0.f, 0.f}, nb_ga[2] = {0.f, 0.f}, nb_be[2] = {0.f, 0.f};
@@ -307,7 +202,7 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     int nb_img = -1, nb_c = -1;
 
     for (int tile = tile_first; tile < tile_end; tile += tile_step) {
-      const TileCoord t = decode_tile(P, tile, MBLK, 128);
+      const TileCoord t = decode_tile(P, tile, 128);
       const int c0 = t.n0 + 16 * e;       // this warp's 16 output channels
       const int ca = c0 + (lane >> 2);    // this thread's channels: ca and ca + 8
       if (has_res && lane == 0) {
@@ -319,7 +214,7 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           tma_load_4d(&tmR, &res_bar[e], my_buf + k * kSwapBox, c0, t.w0, t.h0 + k * rows_per_box, t.img);
         if (nb && tile + tile_step < tile_end) {
           // the NEXT tile's x boxes go to L2 now, so that its loads above are L2 hits
-          const TileCoord tn = decode_tile(P, tile + tile_step, MBLK, 128);
+          const TileCoord tn = decode_tile(P, tile + tile_step, 128);
           for (int k = 0; k < 4; ++k)
             tma_prefetch_4d(&tmR, tn.n0 + 16 * e, tn.w0, tn.h0 + k * rows_per_box, tn.img);
         }
@@ -380,13 +275,6 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         if (rel_b >= 0) mbar_arrive(&b_empty[rel_b]);
         if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
       }
-      if (P.debug & 1) {
-        if (has_res) {
-          mbar_wait(&res_bar[e], res_par);
-          res_par ^= 1;
-        }
-        continue;
-      }
       // accumulator element i: channel ca + 8 ((i >> 1) & 1), pixel 8 (i >> 2) + m2 + (i & 1); in-box pixel and
       // channel of the [32][16] box i >> 4
       auto box_off = [&](int i) { return (i >> 4) * kSwapBox + swz64(8 * ((i >> 2) & 3) + m2 + (i & 1), (lane >> 2) + 8 * ((i >> 1) & 1)); };
@@ -395,7 +283,7 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         return (t.h0 + (p >> tw_shift) < P.H) && (t.w0 + (p & (P.TW - 1)) < P.W);
       };
       // interior tiles need no per-pixel validity test for the GroupNorm / norm-backward sums
-      const bool interior = (t.h0 + MBLK * P.TH <= P.H) && (t.w0 + P.TW <= P.W);
+      const bool interior = (t.h0 + P.TH <= P.H) && (t.w0 + P.TW <= P.W);
       {
         float bias2[2] = {0.f, 0.f};
         if (P.bias_mode == T2H_BIAS_COL) {

@@ -40,28 +40,31 @@ static inline bool pdl_enabled() {
   return on == 1;
 }
 
+// T2H_DEBUG bits; bit 16: CTA 0 of every tap-GEMM / attention launch records a globaltimer trace (t2h_debug_read)
+static inline int debug_bits() {
+  static int bits = -1;
+  if (bits < 0) {
+    const char* e = getenv("T2H_DEBUG");
+    bits = e ? atoi(e) : 0;
+  }
+  return bits;
+}
+
 // Launch a kernel that calls pdl_wait() before its first dependent global access, allowing it to overlap its
 // prologue with the previous kernel's tail (also inside CUDA-graph capture, where it becomes a programmatic edge).
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                                     int cluster_x, Args&&... args) {
+                                     Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute at[2];
+  cudaLaunchAttribute at[1];
   int n = 0;
   if (pdl_enabled()) {
     at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  if (cluster_x > 1) {  // thread-block clusters of cluster_x CTAs along x (grid.x is a multiple of it)
-    at[n].id = cudaLaunchAttributeClusterDimension;
-    at[n].val.clusterDim.x = cluster_x;
-    at[n].val.clusterDim.y = 1;
-    at[n].val.clusterDim.z = 1;
     ++n;
   }
   cfg.attrs = at;

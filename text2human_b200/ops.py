@@ -106,20 +106,12 @@ def _tapgemm(*, a, a_term_imgs, a_imgs, a_bcast, n_img, H, W, a_H, a_W, Cc, a_sw
              b, b_term_g, b_groups, b_batched, n_out, b_sn, b_sg, taps, d, d_mode, d_strides,
              d_plane=0, bias=None, bias_mode=BIAS_NONE, act=ACT_NONE, alpha=1.0, residual=None,
              tile_rows=0, b_groups2=1, b_sg2=0, b_batched_h=0, gn_stats=None, gn_cpg=0, k_split=0, bias_sn=0, a_mn=0, b_mn=0,
-             tap_w=None, accumulate=False, k_partials=0, d_slab=0, a_f32=None, gn=None, nb=None):
+             tap_w=None, accumulate=False, k_partials=0, d_slab=0, nb=None):
     lib = _lib.load()
     Tb = b.shape[0]
     p = TapGemmParams()
-    if a_f32 is not None:
-        # fused GroupNorm(+swish) operand: the kernel normalises the fp32 tensor itself (no planes exist)
-        stats, gamma, beta, eps, swish, groups = gn
-        T = Tb
-        p.a = None; p.a_terms = T; p.a_term_imgs = 0; p.a_imgs = n_img
-        p.a_f32 = a_f32.data_ptr(); p.a_gn_stats = stats.data_ptr(); p.a_gn_gamma = gamma.data_ptr()
-        p.a_gn_beta = beta.data_ptr(); p.a_gn_eps = eps; p.a_gn_swish = 1 if swish else 0; p.a_gn_groups = groups
-    else:
-        T = a.shape[0]
-        p.a = a.data_ptr(); p.a_terms = T; p.a_term_imgs = a_term_imgs; p.a_imgs = a_imgs
+    T = a.shape[0]
+    p.a = a.data_ptr(); p.a_terms = T; p.a_term_imgs = a_term_imgs; p.a_imgs = a_imgs
     p.a_bcast = a_bcast
     p.n_img, p.H, p.W, p.a_H, p.a_W, p.C = n_img, H, W, a_H, a_W, Cc
     p.tile_rows = tile_rows
@@ -130,7 +122,7 @@ def _tapgemm(*, a, a_term_imgs, a_imgs, a_bcast, n_img, H, W, a_H, a_W, Cc, a_sw
     p.ntaps = len(taps)
     for i, (dy, dx, off) in enumerate(taps):
         p.tap_dy[i], p.tap_dx[i], p.tap_img_off[i] = dy, dx, off
-    p.nterms = 3 if (T == 2 and Tb == 2) else 1   # fused operand: T follows the weight planes
+    p.nterms = 3 if (T == 2 and Tb == 2) else 1
     p.d = d.data_ptr(); p.d_mode = d_mode
     p.d_terms = d.shape[0] if d_mode == OUT_PLANES else 0
     p.d_plane = d_plane
@@ -222,51 +214,6 @@ def _stats_for(cout, n, device, want):
 
 
 import os as _os_env
-# Off by default: every slab is rebuilt once per horizontal tap shift (3x the transforms of gn_apply; the 128-byte
-# swizzle phase forbids sub-row views of one slab) by the kernel's producer warps, which made the fused producer slower
-# than the separate gn_apply pass where it was measured.  Kept, parity-tested; T2H_FUSE_GN=1 / set_fuse_gn(True) enable it.
-FUSE_GN = {"on": _os_env.environ.get("T2H_FUSE_GN", "0") == "1"}
-
-
-def set_fuse_gn(on):
-    """fold GroupNorm-apply + swish into the consuming conv's operand producer where the kernel supports it
-    (swapped-operand convs, C % 64 == 0, C <= 256); off: the separate gn_apply pass of round 1.  Returns the old value."""
-    old = FUSE_GN["on"]
-    FUSE_GN["on"] = bool(on)
-    return old
-
-
-def can_fuse_gn(Cin, Cout, W, groups, nchw_out=False, planes_out=False):
-    """mirror of t2h_tapgemm's eligibility test for the fused GroupNorm producer (a 3x3 stride-1 spatial conv)"""
-    if not FUSE_GN["on"] or planes_out or Cin % 64 != 0 or Cin > 256 or Cin % groups != 0 or W < 1:
-        return False
-    return (Cout % 128 == 0 and not nchw_out) or (nchw_out and Cout <= 128)
-
-
-def conv3x3_gn(x, stats, gamma, beta, w, bias, *, eps, swish, groups=32, residual=None, nchw_out=False,
-               want_stats=False):
-    """3x3 conv of swish(GroupNorm(x)) with the normalisation folded into the conv's activation producer.
-    x fp32 NHWC [N,H,W,C] (the previous conv's output), stats its (sum, sumsq) [N,groups,2]; w packed planes
-    [T,9,Cout,C].  Same results, bit for bit, as group_norm(...) followed by conv3x3(...)."""
-    _need_cuda(x, w)
-    N, H, W, Cc = x.shape
-    Cout = w.shape[2]
-    assert w.shape[1] == 9 and w.shape[3] == Cc and x.is_contiguous()
-    st_out, cpg = _stats_for(Cout, N, x.device, want_stats and not nchw_out)
-    if nchw_out:
-        out = torch.empty((N, Cout, H, W), dtype=torch.float32, device=x.device)
-        d_strides = (Cout * H * W, W, 1, H * W)
-    else:
-        out = torch.empty((N, H, W, Cout), dtype=torch.float32, device=x.device)
-        d_strides = (H * W * Cout, W * Cout, Cout, 1)
-    _tapgemm(a=None, a_term_imgs=0, a_imgs=N, a_bcast=0, n_img=N, H=H, W=W, a_H=H, a_W=W, Cc=Cc,
-             a_sw=Cc, a_sh=W * Cc, a_sn=H * W * Cc,
-             b=w, b_term_g=9, b_groups=w.shape[0] * 9, b_batched=0, n_out=Cout, b_sn=Cc, b_sg=Cout * Cc,
-             taps=_TAPS_3x3, d=out, d_mode=OUT_F32, d_strides=d_strides, bias=bias, bias_mode=BIAS_COL,
-             residual=residual, gn_stats=st_out, gn_cpg=cpg, a_f32=x, gn=(stats, gamma, beta, eps, swish, groups))
-    if want_stats:
-        return out, st_out
-    return out
 
 
 def conv3x3(a, w, bias, *, residual=None, planes_out=False, nchw_out=False, want_stats=False, taps=None,
@@ -1107,14 +1054,10 @@ def nb_context(x, stats, gamma, beta, *, act, groups, eps):
     conv would not run on the swapped-operand kernel (channels % 128, narrow images) or T2H_FUSE_NB=0 -- the caller
     then simply omits both arguments and norm_bwd runs its own reduce pass."""
     N, H, W, Cc = x.shape
-    if not FUSE_NB["on"] or Cc % 128 or Cc % groups or H < 2 or os_no_swap() or not x.is_contiguous():
+    if not FUSE_NB["on"] or Cc % 128 or Cc % groups or H < 2 or not x.is_contiguous():
         return None
     sums = torch.zeros((N * Cc * 2,), dtype=torch.float64, device=x.device)
     return dict(x=x, stats=stats, gamma=_f32c(gamma), beta=_f32c(beta), act=act, groups=groups, eps=float(eps), sums=sums)
-
-
-def os_no_swap():
-    return _os_env.environ.get("T2H_NO_SWAP", "0") not in ("", "0")
 
 
 def conv_wgrad(dy, x, taps, dw, *, n, alpha=1.0, k_split=0):

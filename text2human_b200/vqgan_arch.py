@@ -82,16 +82,7 @@ def Normalize(in_channels):
 
 
 def _gn_conv3x3(act, norm, conv, *, residual=None, want_stats=False, nchw_out=False):
-    """swish(GroupNorm(act)) -> 3x3 conv: one fused launch where the kernel supports it (the normalisation happens
-    in the conv's activation producer), else the gn_apply pass followed by the conv"""
-    x = act.x
-    N, H, W, Cc = x.shape
-    Cout = conv.weight.shape[0]
-    if norm.num_groups == ops.GN_GROUPS and ops.can_fuse_gn(Cc, Cout, W, norm.num_groups, nchw_out=nchw_out):
-        stats = act.stats if act.stats is not None else ops.norm_stats(x, norm.num_groups)
-        return ops.conv3x3_gn(x, stats, _f32(norm.weight), _f32(norm.bias), _conv_w(conv), _f32(conv.bias),
-                              eps=norm.eps, swish=True, groups=norm.num_groups, residual=residual,
-                              nchw_out=nchw_out, want_stats=want_stats)
+    """swish(GroupNorm(act)) -> 3x3 conv: the gn_apply pass followed by the conv"""
     a = _gn(act, norm, swish=True, consumer=conv)
     return ops.conv3x3(a, _conv_w(conv), _f32(conv.bias), residual=residual, nchw_out=nchw_out,
                        want_stats=want_stats)

@@ -1,6 +1,4 @@
-"""Time single tapgemm launches (CUDA events, L2-cold via rotating buffers) for a few conv shapes.
-T2H_DEBUG bits isolate pipeline parts (timings only, the results are then wrong): 1 skip epilogue work, 4 skip TMA
-loads."""
+"""Time single tapgemm launches (CUDA events, L2-cold via rotating buffers) for a few conv shapes."""
 import os
 import sys
 
@@ -32,7 +30,6 @@ def bench_conv(N, H, W, Cin, Cout, terms, residual, stats, iters=5):
     return ms, fl / ms / 1e9
 
 
-print("T2H_DEBUG =", os.environ.get("T2H_DEBUG", "0"))
 for (N, H, W, Ci, Co) in [(16, 512, 256, 128, 128), (16, 128, 64, 256, 256), (16, 64, 32, 256, 256),
                           (16, 32, 16, 512, 512)]:
     for terms in (1, 2):
