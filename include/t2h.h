@@ -438,6 +438,15 @@ int t2h_vq_bwd(const float* z, const float* codebook, const int64_t* idx, const 
 /* sum[0] += sum |x - xrec|; grad (may be NULL) = gscale * sign(xrec - x)   (torch.abs, vqgan_model.py:449) */
 int t2h_l1_loss(const float* x, const float* xrec, float* grad, double* sum, int64_t n, float gscale,
                 t2h_stream_t stream);
+/* BCE-with-logits against a one-hot target that is never materialised (BCELossWithQuant, segmentation_loss.py:12-25,
+ * target F.one_hot(segm) of VQSegmentationModel.feed_data, vqgan_model.py:117-124).  logits fp32 NHWC [n][h][w][c];
+ * ids float [n][1][h][w], the class-id convention of t2h_onehot_to_planes (a non-integer or out-of-range id gives an
+ * all-zero target row).  One pass: loss_sum[0] += sum max(x,0) - x t + log1p(exp(-|x|)); grad_planes (may be NULL)
+ * = fp16 planes [terms][n][h][w][c_pad] of gscale (sigmoid(x) - t), pad channels 0 -- the output-gradient operand
+ * of the decoder's conv_out; colsum (may be NULL) [c] += column sums of that gradient -- conv_out's bias gradient.
+ * c % 4 == 0, c_pad % 8 == 0, c_pad <= 256. */
+int t2h_bce_logits(const float* logits, const float* ids, int n, int h, int w, int c, int c_pad, float gscale,
+                   double* loss_sum, void* grad_planes, int terms, float* colsum, t2h_stream_t stream);
 /* sgn = +1 / -1: sum += relu(1 - sgn*l), grad = -sgn*gscale where positive (hinge_d_loss, vqgan_loss.py:21-26);
  * sgn = 0: sum += l, grad = gscale (g_loss = -mean(logits_fake), vqgan_model.py:461) */
 int t2h_hinge_loss(const float* logits, float* grad, double* sum, int64_t n, float sgn, float gscale,

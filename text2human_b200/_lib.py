@@ -115,6 +115,7 @@ SIGNATURES = {
     "t2h_planes_s2d": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),
     "t2h_vq_bwd": (_I, [_P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _F, _F, _P]),
     "t2h_l1_loss": (_I, [_P, _P, _P, _P, _L, _F, _P]),
+    "t2h_bce_logits": (_I, [_P, _P, _I, _I, _I, _I, _I, _F, _P, _P, _I, _P, _P]),
     "t2h_hinge_loss": (_I, [_P, _P, _P, _L, _F, _F, _P]),
     "t2h_diffaug_fwd": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "t2h_diffaug_bwd": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),

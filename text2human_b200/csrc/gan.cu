@@ -309,6 +309,77 @@ __global__ void l1_kernel(const float* __restrict__ x, const float* __restrict__
   block_add(acc, sum);
 }
 
+// BCE-with-logits against the one-hot of a class-id map (BCELossWithQuant, segmentation_loss.py:12-25, with the target
+// of VQSegmentationModel.feed_data, vqgan_model.py:117-124).  Per element x, t = [c == id(pixel)]:
+//   loss += max(x,0) - x t + log1p(exp(-|x|)),   g = gscale (sigmoid(x) - t)
+// g goes straight to fp16 hi/lo planes [terms][pix][c_pad] (pad channels 0) and its column sums to colsum[c].
+// A thread owns 8 channels of one pixel (two float4 loads, one 16-byte store per plane); blockDim is a multiple of
+// c_pad/8, so a thread meets the same 8 channels at every pixel and keeps their column sums in registers.
+// sigmoid(x) - 1 is formed as -sigmoid(-x), so saturated logits keep their tiny gradients.
+__global__ void bce_logits_kernel(const float* __restrict__ x, const float* __restrict__ ids, long long npix, int C,
+                                  int c_pad, float gscale, double* __restrict__ loss, __half* __restrict__ planes,
+                                  int terms, float* __restrict__ colsum) {
+  extern __shared__ double cs_sm[];  // [c_pad]: the block's column sums
+  const int c8 = c_pad >> 3;
+  const int lanes = blockDim.x / c8;
+  const int c0 = (threadIdx.x % c8) * 8;
+  const int lane = threadIdx.x / c8;
+  const long long plane = npix * c_pad;
+  for (int c = threadIdx.x; c < c_pad; c += blockDim.x) cs_sm[c] = 0.0;
+  __syncthreads();
+  float cs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  double acc = 0.0;
+  if (lane < lanes) {
+    for (long long p = (long long)blockIdx.x * lanes + lane; p < npix; p += (long long)gridDim.x * lanes) {
+      const float v = __ldg(ids + p);
+      const int cls = (v == floorf(v) && v >= 0.f && v < (float)C) ? (int)v : -1;
+      float xs[8];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (c0 + 4 * h < C) q = __ldg(reinterpret_cast<const float4*>(x + p * C + c0 + 4 * h));
+        xs[4 * h + 0] = q.x;
+        xs[4 * h + 1] = q.y;
+        xs[4 * h + 2] = q.z;
+        xs[4 * h + 3] = q.w;
+      }
+      H8 hi, lo;
+      float part = 0.f;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int c = c0 + e;
+        float g = 0.f;
+        if (c < C) {
+          const float xv = xs[e];
+          const float en = expf(-fabsf(xv));
+          const float r = 1.f / (1.f + en);
+          const float sp = xv >= 0.f ? r : en * r;   // sigmoid(x)
+          const float sn = xv >= 0.f ? en * r : r;   // sigmoid(-x) = 1 - sigmoid(x)
+          const bool t = c == cls;
+          part += fmaxf(xv, 0.f) - (t ? xv : 0.f) + log1pf(en);
+          g = gscale * (t ? -sn : sp);
+          cs[e] += g;
+        }
+        split_f16(g, hi.v[e], lo.v[e]);
+      }
+      acc += (double)part;
+      if (planes) {
+        *reinterpret_cast<H8*>(planes + p * c_pad + c0) = hi;
+        if (terms == 2) *reinterpret_cast<H8*>(planes + plane + p * c_pad + c0) = lo;
+      }
+    }
+  }
+  if (colsum) {
+    if (lane < lanes) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) atomicAdd(&cs_sm[c0 + e], (double)cs[e]);
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < C; c += blockDim.x) atomicAdd(&colsum[c], (float)cs_sm[c]);
+  }
+  block_add(acc, loss);
+}
+
 // hinge term: sum += relu(1 - sgn*l); grad = -sgn*gscale where 1 - sgn*l > 0   (hinge_d_loss, vqgan_loss.py:21-26)
 // sgn = 0: plain sum of l (g_loss = -mean(logits_fake)) with constant gradient gscale
 __global__ void hinge_kernel(const float* __restrict__ l, float* __restrict__ grad, double* __restrict__ sum,
@@ -593,6 +664,21 @@ int t2h_l1_loss(const float* x, const float* xrec, float* grad, double* sum, int
                 t2h_stream_t stream) {
   T2H_CHECK_ARG(x && xrec && sum && n > 0, "l1_loss: bad args");
   l1_kernel<<<grid_cap(n, 256, 4), 256, 0, as_stream(stream)>>>(x, xrec, grad, sum, n, gscale);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_bce_logits(const float* logits, const float* ids, int n, int h, int w, int c, int c_pad, float gscale,
+                   double* loss_sum, void* grad_planes, int terms, float* colsum, t2h_stream_t stream) {
+  T2H_CHECK_ARG(logits && ids && loss_sum && n > 0 && h > 0 && w > 0 && c > 0, "bce_logits: bad args");
+  T2H_CHECK_ARG(c % 4 == 0 && c_pad >= c && c_pad % 8 == 0 && c_pad <= 256, "bce_logits: c=%d c_pad=%d", c, c_pad);
+  T2H_CHECK_ARG(!grad_planes || terms == 1 || terms == 2, "bce_logits: terms=%d", terms);
+  const long long npix = (long long)n * h * w;
+  const int c8 = c_pad / 8;
+  // whole warps (block_add) and a whole number of pixels per block (fixed channels per thread)
+  const int block = 32 * c8 * (c8 < 8 ? 8 / c8 : 1);
+  bce_logits_kernel<<<grid_cap(npix, block / c8, 4), block, c_pad * sizeof(double), as_stream(stream)>>>(
+      logits, ids, npix, c, c_pad, gscale, loss_sum, reinterpret_cast<__half*>(grad_planes), terms, colsum);
   T2H_LAUNCH_OK();
   return T2H_OK;
 }

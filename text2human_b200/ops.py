@@ -1217,6 +1217,25 @@ def l1_loss(x, xrec, sum_out, gscale=0.0, want_grad=True):
     return grad
 
 
+def bce_logits(logits, segm, sum_out, gscale=1.0, want_grad=True, colsum_out=None, terms=None):
+    """BCE-with-logits of fp32 NHWC ``logits`` [N,H,W,C] against the one-hot of the class-id map ``segm`` (float
+    [N,1,H,W], the ids onehot_to_planes reads; a non-integer or out-of-range id has an all-zero target row):
+    sum_out[0] += the loss summed over all N*C*H*W elements; -> fp16 planes [T,N,H,W,c_pad] of
+    gscale * (sigmoid(logits) - onehot) (or None); ``colsum_out`` [C] += the column sums of that gradient"""
+    _need_cuda(logits, segm, sum_out)
+    segm = _f32c(segm)
+    N, H, W, Cc = logits.shape
+    assert logits.is_contiguous() and logits.dtype == torch.float32 and segm.numel() == N * H * W
+    assert sum_out.dtype == torch.float64 and (colsum_out is None or colsum_out.numel() == Cc)
+    terms = terms or get_terms()
+    cp = (Cc + 7) // 8 * 8
+    planes = torch.empty((terms, N, H, W, cp), dtype=torch.float16, device=logits.device) if want_grad else None
+    _count(1)
+    _lib.check(_lib.load().t2h_bce_logits(_ptr(logits), _ptr(segm), N, H, W, Cc, cp, gscale, _ptr(sum_out),
+                                          _ptr(planes), terms, _ptr(colsum_out), _stream()))
+    return planes
+
+
 def hinge_loss(logits, sum_out, sgn, gscale=0.0, want_grad=True):
     _need_cuda(logits)
     assert logits.is_contiguous()

@@ -563,16 +563,19 @@ class VectorQuantizer(nn.Module):
         r["loss"] = _loss_from_sqerr(r["sqerr"], z.numel(), self.beta)
         return r
 
-    @torch.no_grad()
     def forward(self, z, temp=None, rescale_logits=False, return_logits=False):
         _check_gumbel_args(temp, rescale_logits, return_logits)
-        zh = ops.nchw_to_nhwc(z)
-        r = ops.vq_search(zh, self._codebook(), None, want_list=False, want_nhwc=False)
-        loss = _loss_from_sqerr(r["sqerr"], z.numel(), self.beta)
-        idx = r["idx"]
-        if not self.sane_index_shape:
-            idx = idx.reshape(-1)
-        return r["zq_nchw"], loss, (None, None, idx)
+        from . import vqgan_autograd as VA
+        if VA.recording(self, z):          # training: straight-through + codebook-loss gradients
+            return VA.quantizer_forward(self, z)
+        with torch.no_grad():
+            zh = ops.nchw_to_nhwc(z)
+            r = ops.vq_search(zh, self._codebook(), None, want_list=False, want_nhwc=False)
+            loss = _loss_from_sqerr(r["sqerr"], z.numel(), self.beta)
+            idx = r["idx"]
+            if not self.sane_index_shape:
+                idx = idx.reshape(-1)
+            return r["zq_nchw"], loss, (None, None, idx)
 
     @torch.no_grad()
     def get_codebook_entry(self, indices, shape):

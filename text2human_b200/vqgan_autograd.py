@@ -119,6 +119,9 @@ def _pow2_scale(dy, target=64.0):
     hi/lo planes (absolute resolution 2^-24), so every node rescales its incoming gradient to ~``target`` by a power
     of two and divides what it returns (one device->host read per node; the native trainer uses static scales)."""
     amax = float(dy.abs().max())
+    # (the Encoder and Decoder-trunk nodes use target 1, the magnitude the native trainers' loss scales give: over
+    # their ~20 layers the gradient grows, and the attention backward near the far end writes 2^8-scaled score
+    # gradients to fp16 planes, which overflowed for the parsing tokenizer's gradients at target 64)
     if not (amax > 0.0) or amax != amax or amax == float("inf"):
         return 1.0
     import math
@@ -226,7 +229,7 @@ class _EncoderFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dz):
         inl, body, out = ctx.layers
-        s = _pow2_scale(dz)
+        s = _pow2_scale(dz, target=1.0)
         with torch.no_grad(), _Replayable(ctx.host, [inl, body, out]) as rp:
             g = ops.nchw_to_nhwc((dz * s).contiguous())
             inl.bwd(body.bwd(out.bwd(g)))
@@ -262,7 +265,7 @@ class _DecTrunkFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dh):
         inl, body = ctx.layers
-        s = _pow2_scale(dh)
+        s = _pow2_scale(dh, target=1.0)
         with torch.no_grad(), _Replayable(ctx.host, [inl, body]) as rp:
             g = inl.bwd(body.bwd(VT.Grad((dh * s).contiguous())))
             dz = ops.nhwc_to_nchw(g.g)
@@ -339,6 +342,44 @@ class _VQTexFn(torch.autograd.Function):
 def quantizer_texture_forward(q, z, segm_map):
     zq, loss, cont, lst = _VQTexFn.apply(q, z, segm_map, *[e.weight for e in q.embedding_list])
     return zq, loss, (None, cont, list(lst.unbind(0)))
+
+
+# ----------------------------------------------------------------------------
+# VectorQuantizer (one codebook; straight-through + beta codebook loss, vqgan_arch.py:79-122)
+# ----------------------------------------------------------------------------
+class _VQFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, z, weight):
+        with torch.no_grad():
+            zh = ops.nchw_to_nhwc(z.detach().float().contiguous())
+            cb = weight.detach().float().unsqueeze(0).contiguous()
+            r = ops.vq_search(zh, cb, None, want_list=False, want_nhwc=False)
+            loss = ((1.0 + q.beta) * r["sqerr"][0] / zh.numel()).to(torch.float32)
+        ctx.q, ctx.saved_vq = q, (zh, cb, r["idx"])
+        ctx.mark_non_differentiable(r["idx"])
+        return r["zq_nchw"], loss, r["idx"]
+
+    @staticmethod
+    def backward(ctx, dzq, dloss, _):
+        zh, cb, idx = ctx.saved_vq
+        nel = zh.numel()
+        dl = float(dloss) if dloss is not None else 0.0
+        # legacy: loss = mean((zq.detach()-z)^2) + beta*mean((zq-z.detach())^2); otherwise beta weighs the z term
+        w_z, w_e = (1.0, ctx.q.beta) if ctx.q.legacy else (ctx.q.beta, 1.0)
+        with torch.no_grad():
+            s = _pow2_scale(dzq) if dzq is not None else 1.0
+            dzq_h = ops.nchw_to_nhwc((dzq * s).contiguous()) if dzq is not None else None
+            dcb = torch.zeros_like(cb)
+            dz = ops.vq_bwd(zh, cb, idx, None, dzq_h, dcb, 2.0 * w_z * dl * s / nel, 2.0 * w_e * dl * s / nel)
+            dzn = ops.nhwc_to_nchw(dz)
+        grads = _unscale([dzn, dcb], s)
+        return None, grads[0], grads[1][0]
+
+
+def quantizer_forward(q, z):
+    """-> (z_q, loss, (None, None, idx)) as VectorQuantizer.forward; idx flat unless ``sane_index_shape``"""
+    zq, loss, idx = _VQFn.apply(q, z, q.embedding.weight)
+    return zq, loss, (None, None, idx if q.sane_index_shape else idx.reshape(-1))
 
 
 def recording(module, *tensors):

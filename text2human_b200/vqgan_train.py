@@ -327,13 +327,19 @@ class NormConvOutL(Layer):
 
     def bwd(self, dy, gw_known=None):
         """``gw_known``: the conv's weight gradient for ``dy`` when the caller already has it (the trainer: by
-        linearity from the adaptive weight's two gradients) -- it is added instead of being recomputed"""
+        linearity from the adaptive weight's two gradients) -- it is added instead of being recomputed.  ``dy`` may
+        be a Grad that already holds the planes and column sums (the segm tokenizer's fused BCE loss kernel)."""
         x, st, a, N, H, W = self.saved.pop()
         cp = self.cp(self.conv)
-        dyp = self._dy_planes(dy)
-        if cp.gb is not None:
-            g2 = ops.nchw_to_nhwc(dy) if self.nchw else dy
-            ops.colsum_(cp.gb[:cp.co], g2.reshape(-1, cp.co))
+        if isinstance(dy, Grad):
+            dyp = dy.p
+            if cp.gb is not None:
+                ops.add_inplace(cp.gb[:cp.co], dy.colsum)
+        else:
+            dyp = self._dy_planes(dy)
+            if cp.gb is not None:
+                g2 = ops.nchw_to_nhwc(dy) if self.nchw else dy
+                ops.colsum_(cp.gb[:cp.co], g2.reshape(-1, cp.co))
         if gw_known is not None:
             cp.gw.add_(gw_known)
         else:
@@ -599,7 +605,9 @@ def backward_order(model, disc=None):
                 order += attn(lvl.attn[i_block])
             order += res(lvl.block[i_block])
     order += res(dec.mid.block_2) + attn(dec.mid.attn_1) + res(dec.mid.block_1) + [dec.conv_in]
-    order += [model.post_quant_conv] + list(model.quantize.embedding_list) + [model.quant_conv]
+    q = model.quantize
+    books = list(q.embedding_list) if hasattr(q, "embedding_list") else [q.embedding]   # texture | plain quantizer
+    order += [model.post_quant_conv] + books + [model.quant_conv]
     order += [enc.conv_out, enc.norm_out] + res(enc.mid.block_2) + attn(enc.mid.attn_1) + res(enc.mid.block_1)
     for i_level in reversed(range(enc.num_resolutions)):
         lvl = enc.down[i_level]
