@@ -201,7 +201,7 @@ __global__ void gn_stats_kernel(const float* __restrict__ x, double* __restrict_
       s[2] += v.z; ss[2] += v.z * v.z;
       s[3] += v.w; ss[3] += v.w * v.w;
     }
-    if (cpg >= 4) {
+    if (cpg % 4 == 0) {  // the float4 lies inside one group; with cpg = 5, 6, 10, ... it can straddle two
       const int g = (cs * 4) / cpg;
       atomicAdd(&sm[g], (s[0] + s[1]) + (s[2] + s[3]));
       atomicAdd(&sm[groups + g], (ss[0] + ss[1]) + (ss[2] + ss[3]));

@@ -877,6 +877,8 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
   P.d_term_imgs = 0;
 
   // ---- tile shape
+  // (tests/test_gpu_tapgemm_paths.py::route restates the selection below, tile shape to epilogue mode, and labels its
+  // cases with it: a routing change updates it in the same change)
   // one 128-row block = TH x TW output positions of one image
   int TW, TH;
   if (p->H == 1 || p->tile_rows) {
