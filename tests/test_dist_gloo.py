@@ -76,22 +76,23 @@ def _train_worker(rank, world, port, q):
     D.init("gloo")
     cfg = dict(R.TINY_TRANSFORMER, bert_n_layers=5)
     tr = SamplerTrainer(TransformerMultiHead(**cfg), bucket_layers=2)
-    n = tr.flat_g.numel()
-    tr.flat_g.copy_(torch.arange(n, dtype=torch.float32) % 97 + 1000.0 * rank)
-    # the order the backward pass finishes the buckets in: head, blocks last to first, embeddings
-    tr._bucket_done("head", True)
+    sp, m = tr.space, tr.m
+    n = sp.flat_g.numel()
+    sp.flat_g.copy_(torch.arange(n, dtype=torch.float32) % 97 + 1000.0 * rank)
+    # the modules the backward pass reports finished: head, blocks last to first, embeddings
+    sp.arm(True)
+    sp.done(m.ln_f)
     for li in range(4, -1, -1):
-        if li % tr.bucket_layers == 0:
-            tr._bucket_done((li, min(5, li + tr.bucket_layers)), True)
-    tr._bucket_done("emb", True)
-    n_handles = len(tr._handles)
-    tr.wait_reduced()
+        sp.done(m.blocks[li].ln1)
+    sp.done(m.texture_emb)
+    n_handles = len(sp.handles)
+    sp.wait()
     if rank == 0:
-        q.put((tr.flat_g.numpy().tolist(), n_handles))
+        q.put((sp.flat_g.numpy().tolist(), n_handles))
     torch.distributed.destroy_process_group()
 
 
-def test_trainer_gradient_buckets_cover_flat_buffer_gloo():
+def test_sampler_flat_store_buckets_cover_flat_buffer_gloo():
     port = _free_port()
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
@@ -140,20 +141,18 @@ def _vqgan_worker(rank, world, port, q):
     for name, sp in (("gen", tr.gen), ("dsc", tr.dsc)):
         n = sp.flat_g.numel()
         sp.flat_g.copy_(torch.arange(n, dtype=torch.float32) % 97 + 1000.0 * rank)
-        tr._handles = []
-        tr._arm(sp, True)
+        sp.arm(True)
         for mod, _, _ in sp.mod_span:                   # the order the backward pass finishes the modules in
-            tr.done(mod)
-        n_handles = len(tr._handles)
-        tr.wait_reduced()
-        tr._reduce = False
+            sp.done(mod)
+        n_handles = len(sp.handles)
+        sp.wait()
         want = 2 * (torch.arange(n, dtype=torch.float32) % 97) + 1000.0     # every element summed exactly once
         out[name] = (bool(torch.equal(sp.flat_g, want)), n_handles, len(sp.buckets))
     q.put((rank, psum, same_as_built, out if rank == 0 else None, tuple(m.decoder.conv_out.weight.shape)))
     torch.distributed.destroy_process_group()
 
 
-def test_vqgan_trainer_broadcast_and_gradient_buckets_gloo():
+def test_vqgan_flat_stores_broadcast_and_gradient_buckets_gloo():
     port = _free_port()
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

@@ -47,7 +47,7 @@ def _worker(rank, world, port, q):
     x, mask = R.image(7, world, 3, 64, 32), R.blocky_mask(8, world, 64, 32, 8)
     tr.aug_draw_fn = _draws(5, 2 * rank)                     # 2 DiffAugment calls (fake, real) per image
     tr.training_step(dict(image=x[rank:rank + 1], texture_mask=mask[rank:rank + 1]), 3)
-    n_reduces = len(tr._handles)
+    n_reduces = len(tr.gen.handles) + len(tr.dsc.handles)
     tr.wait_reduced()
     torch.cuda.synchronize()
     g_gen, g_dsc = tr.gen.flat_g.clone(), tr.dsc.flat_g.clone()
@@ -59,7 +59,6 @@ def _worker(rank, world, port, q):
         # the single-process reference on the same device: both images as two micro-batches
         m1, disc1, _ = build(dev)
         t1 = VQGANTrainer(m1, disc1, micro_batch=1)
-        t1._handles = []
         t1.aug_draw_fn = _draws(5, 0)
         t1.force_no_reduce = True
         t1.training_step(dict(image=x, texture_mask=mask), 3)

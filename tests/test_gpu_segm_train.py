@@ -313,8 +313,8 @@ def _worker(rank, world, port, out_dir):
     dist.init_process_group("nccl", device_id=dev)
     tr = SegmTokenizerTrainer(build(dev), bucket_bytes=256 << 10)      # several buckets even for the reduced net
     tr.training_step(dict(segm=segm[rank:rank + 1]))
-    out["n_reduces"], out["n_buckets"] = len(tr._handles), len(tr.space.buckets)
-    tr.wait_reduced()
+    out["n_reduces"], out["n_buckets"] = len(tr.space.handles), len(tr.space.buckets)
+    tr.space.wait()
     g = tr.space.flat_g.clone()
     tr.adam_step()
     torch.cuda.synchronize()

@@ -38,7 +38,7 @@ def test_train_loss_restatement_matches_reference_fixture():
         assert ((p1 - p.detach()) - d_want).abs().max() <= 2e-3 * 1e-4 + 1e-9, k
 
 
-def test_trainer_flat_layout_aliases_parameters():
+def test_sampler_flat_store_layout_aliases_parameters():
     from text2human_b200.transformer_train import SamplerTrainer, targets_from_gt_list
     cfg, net, sd, (x_0, gt_list, segm, tex), gold = _setup()
     net.load_state_dict(sd, strict=True)
@@ -52,17 +52,17 @@ def test_trainer_flat_layout_aliases_parameters():
     # q|k|v weights and biases are adjacent so that one GEMM produces all three gradients
     a = net.blocks[0].attn
     C = cfg["bert_n_emb"]
-    wqkv = tr._flat_view(tr.flat_p, a.query.weight, 3 * C, C)
+    wqkv, _ = tr.space.joint([a.query.weight, a.key.weight, a.value.weight], C)
     assert torch.equal(wqkv, torch.cat((a.query.weight, a.key.weight, a.value.weight), 0))
-    bqkv = tr._flat_view(tr.flat_p, a.query.bias, 1, 3 * C)[0]
+    bqkv, _ = tr.space.joint([a.query.bias, a.key.bias, a.value.bias])
     assert torch.equal(bqkv, torch.cat((a.query.bias, a.key.bias, a.value.bias), 0))
-    wh = tr._flat_view(tr.flat_p, net.head_list[0].weight, cfg["codebook_size"], C)
+    wh, _ = tr.space.joint([h.weight for h in net.head_list], C)
     assert torch.equal(wh, torch.cat([h.weight for h in net.head_list], 0))
     # gradient views alias the flat gradient buffer; buckets tile it without gaps
-    tr.flat_g.fill_(3.0)
+    tr.space.flat_g.fill_(3.0)
     assert all(float(p.grad.min()) == 3.0 for p in net.parameters())
-    spans = sorted(tr.group_span.values())
-    assert spans[0][0] == 0 and spans[-1][1] == tr.flat_g.numel()
+    spans = sorted(tr.space.buckets)
+    assert spans[0][0] == 0 and spans[-1][1] == tr.space.flat_g.numel()
     assert all(spans[i][1] == spans[i + 1][0] for i in range(len(spans) - 1))
     own = targets_from_gt_list(gt_list)
     assert torch.equal(own + 16 * tex, x_0)

@@ -29,6 +29,11 @@ def init(backend=None, device=None):
     return rank, local_rank, world
 
 
+def world_size():
+    """ranks in the default process group (1 without one)"""
+    return dist.get_world_size() if dist.is_initialized() else 1
+
+
 def shard_range(n_items, rank, world):
     """Contiguous, balanced [start, stop) slice of n_items for `rank` (first n_items % world ranks get
     one extra item); empty for ranks beyond n_items."""

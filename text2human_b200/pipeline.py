@@ -279,7 +279,7 @@ class Sampler(nn.Module):
     @property
     def _graphs(self):
         """captured graphs live ON the transformer module (next to its packed-weight cache) so that whoever
-        invalidates the packed weights (``SamplerTrainer._drop_packed_caches``) drops them too"""
+        invalidates the packed weights (``flat_params.drop_packed_caches``) drops them too"""
         return self.sampler_fn.__dict__.setdefault("_t2h_graphs", {})
 
     def _weights_signature(self):

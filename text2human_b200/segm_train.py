@@ -13,8 +13,8 @@ reference's ``training_step`` + ``loss.backward()`` + ``optimizer.step()``:
     attention backward) and ``vq_search`` / ``vq_bwd`` for the quantizer;
   * loss: ``bce_logits`` reads the decoder's NHWC logits and the ids once and writes the output gradient as the
     fp16 planes conv_out's gradients read, plus conv_out's bias gradient (DESIGN §4.4);
-  * parameters, gradients and Adam moments in one flat buffer; gradient buckets are all-reduced over the default
-    process group while the backward pass runs, as in ``VQGANTrainer``.
+  * parameters, gradients and Adam moments in one ``flat_params.ParamSpace``, whose gradient buckets are all-reduced
+    over the default process group while the backward pass runs, as in ``VQGANTrainer``.
 
 The drop-in path for the same step (the reference's own ``optimize_parameters`` on the arch mirrors) goes through
 the autograd nodes of ``vqgan_autograd``.
@@ -24,12 +24,14 @@ import io
 import math
 
 import torch
-import torch.distributed as dist
 import torch.nn as nn
 
 from . import conv_grad as G
 from . import ops
 from . import vqgan_train as VT
+from .dist import world_size
+from .flat_params import ParamSpace, drop_packed_caches, load_checkpoint, save_checkpoint
+from .vqgan_train import NETS
 from .vqgan_arch import Decoder, Encoder, VectorQuantizer
 
 
@@ -67,9 +69,6 @@ class ConvInPlanesL(VT.ConvInImageL):
         return VT.Act(y, st)
 
 
-NETS = ("encoder", "decoder", "quantize", "quant_conv", "post_quant_conv")
-
-
 class SegmTokenizerTrainer:
     """Owns a model with ``encoder``, ``decoder``, ``quantize`` (VectorQuantizer), ``quant_conv``,
     ``post_quant_conv`` (e.g. ``SegmTokenizerModel``); ``optimize_parameters(data)`` is one reference training step
@@ -90,16 +89,12 @@ class SegmTokenizerTrainer:
         self.dec_in, self.dec_body, _ = VT.decoder_layers(self, dec)
         self.dec_out = VT.NormConvOutL(self, dec.norm_out, dec.conv_out, nchw=False)     # logits NHWC
         self.qconv, self.pqconv = VT.Lin1x1L(self, model.quant_conv), VT.Lin1x1L(self, model.post_quant_conv)
-        self.space = VT.ParamSpace(VT.backward_order(model), self.device, bucket_bytes)
-        w = q.embedding.weight
-        n_e, D = w.shape
-        off = self.space.g(w).storage_offset()
-        self.codebook = self.space.flat_p[off:off + n_e * D].view(1, n_e, D)
-        self.g_codebook = self.space.flat_g[off:off + n_e * D].view(1, n_e, D)
-        self._handles = []
-        self._reduce = False
+        self.space = ParamSpace(VT.backward_order(model), self.device, bucket_bytes)
+        n_e, D = q.embedding.weight.shape
+        cb, gcb = self.space.joint([q.embedding.weight], D)
+        self.codebook, self.g_codebook = cb.view(1, n_e, D), gcb.view(1, n_e, D)
         self._out = None
-        self.space.sync_from_rank0()
+        self._sync_from_rank0()
 
     # ---- plumbing used by the layers
     def space_of(self, mod):
@@ -108,24 +103,9 @@ class SegmTokenizerTrainer:
     def space_of_param(self, p):
         return self.space
 
-    def done(self, mod):
-        """all gradients of ``mod`` are final: if it closes a bucket, start that bucket's all-reduce (asynchronously)
-        while the backward pass continues"""
-        if not self._reduce:
-            return
-        b = self.space.bucket_last.get(mod)
-        if b is not None:
-            a, e = self.space.buckets[b]
-            self._handles.append(dist.all_reduce(self.space.flat_g[a:e], op=dist.ReduceOp.SUM, async_op=True))
-
-    def wait_reduced(self):
-        for h in self._handles:
-            h.wait()
-        self._handles = []
-
-    @staticmethod
-    def _world():
-        return dist.get_world_size() if dist.is_initialized() else 1
+    def _sync_from_rank0(self):
+        self.space.sync_from_rank0()
+        drop_packed_caches(self.model)
 
     # ---- one step
     def training_step(self, data):
@@ -143,7 +123,6 @@ class SegmTokenizerTrainer:
         S = self.loss_scale = 2.0 ** math.floor(math.log2(nel))
         sp, dev = self.space, self.device
         sp.flat_g.zero_()
-        self._handles = []
         sp.prepare(ops.get_terms())
         h = self.enc_out.fwd(self.enc_body.fwd(self.enc_in.fwd(ops.onehot_to_planes(segm, C))))
         z = self.qconv.fwd(h)
@@ -156,7 +135,7 @@ class SegmTokenizerTrainer:
         cs = torch.zeros(C, dtype=torch.float32, device=dev)
         dlp = ops.bce_logits(logits, segm, bce, gscale=S / nel, colsum_out=cs)
         del logits
-        self._reduce = self._world() > 1
+        sp.arm(True)
         g = self.dec_in.bwd(self.dec_body.bwd(self.dec_out.bwd(VT.Grad(None, dlp, cs))))
         g = self.pqconv.bwd(g)
         # codebook loss (legacy beta placement, vqgan_arch.py:98-103): coef_z on (z - e), coef_e on (e - z)
@@ -164,12 +143,9 @@ class SegmTokenizerTrainer:
         zn = z.numel()
         dz = ops.vq_bwd(z, self.codebook, r["idx"], None, g.g, self.g_codebook, 2.0 * w_z * S / zn,
                         2.0 * w_e * S / zn)
-        self.done(self.model.quantize.embedding)
+        sp.done(self.model.quantize.embedding)
         g = self.qconv.bwd(VT.Grad(dz))
         self.enc_in.bwd(self.enc_body.bwd(self.enc_out.bwd(g.g)))
-        if self._reduce:
-            assert len(self._handles) == len(sp.buckets), (len(self._handles), len(sp.buckets))
-        self._reduce = False
         sp.release()
         self._out = dict(bce=bce, sqerr=r["sqerr"], nel=nel, z_numel=zn, idx=r["idx"])
         return self._out
@@ -182,10 +158,9 @@ class SegmTokenizerTrainer:
         return dict(total_loss=bce + quant, bce_loss=bce, quant_loss=quant)
 
     def adam_step(self):
-        self.wait_reduced()
-        self.space.adam(self.lr, self.betas, self.eps, 1.0 / (self._world() * self.loss_scale))
-        for mod in self.model.modules():       # packed-weight caches of the mirrors' inference path
-            mod.__dict__.pop("_t2h_cache", None)
+        self.space.wait()
+        self.space.adam(self.lr, self.betas, self.eps, 1.0 / (world_size() * self.loss_scale))
+        drop_packed_caches(self.model)
 
     def optimize_parameters(self, data):
         self.training_step(data)
@@ -193,18 +168,14 @@ class SegmTokenizerTrainer:
 
     # ---- checkpoint / resume: the reference layout (what load_pretrained_segm_token reads, sample_model.py:154-166)
     # plus the optimiser state
+    def _nets(self):
+        return {k: getattr(self.model, k) for k in NETS}
+
     def save(self, path):
-        m = self.model
-        net = {k: {kk: vv.detach().clone().contiguous() for kk, vv in getattr(m, k).state_dict().items()}
-               for k in NETS}
-        torch.save(dict(net, optimizer=self.space.state()), path)
+        save_checkpoint(path, self._nets(), self.space.state())
 
     def load(self, path):
-        ck = torch.load(path, map_location=self.device)
-        for k in NETS:
-            getattr(self.model, k).load_state_dict(ck[k], strict=True)
-        if "optimizer" in ck:
-            self.space.load_state(ck["optimizer"])
-        for mod in self.model.modules():
-            mod.__dict__.pop("_t2h_cache", None)
-        self.space.sync_from_rank0()
+        opt = load_checkpoint(path, self._nets(), self.device)
+        if opt is not None:
+            self.space.load_state(opt)
+        self._sync_from_rank0()

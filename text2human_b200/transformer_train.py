@@ -7,17 +7,19 @@ re-weighted ELBO, ``loss.backward()``, ``torch.optim.Adam.step()``) for the ``Tr
 mirror.  Forward and backward contractions (dgrad, wgrad, attention gradients) all run on
 ``t2h_tapgemm``; a gradient GEMM that contracts over the rows of a stored matrix (dY^T X, P^T dY, dY W) reads it
 as an MN-major tensor-core operand (``a_mn`` / ``b_mn``), so no transposed copy of any activation, gradient or
-weight is made.  Parameters, gradients and Adam moments live in flat
-fp32 buffers (the ``nn.Parameter``s are views), so the optimiser is one kernel launch and the gradient
-all-reduce works on contiguous buckets that are launched as soon as the backward pass has finished the
-layers they cover (overlap with the remaining backward).
+weight is made.  Parameters, gradients and Adam moments live in a ``flat_params.ParamSpace`` (the
+``nn.Parameter``s are views of its flat fp32 buffers), so the optimiser is one kernel launch and the gradient
+all-reduce works on contiguous buckets (the heads with ``ln_f``, each run of ``bucket_layers`` blocks, the
+embeddings) that are launched as soon as the backward pass has finished the layers they cover (overlap with the
+remaining backward).
 """
 import math
 
 import torch
-import torch.distributed as dist
 
 from . import ops
+from .dist import world_size
+from .flat_params import ParamSpace, drop_packed_caches
 
 
 def targets_from_gt_list(gt_list):
@@ -39,88 +41,51 @@ class SamplerTrainer:
         self.num_timesteps = num_timesteps
         self.mask_id = model.codebook_size if mask_id is None else mask_id
         self.loss_type = loss_type
-        self.step_count = 0
         self.loss_scale = 1.0
         self.bucket_layers = bucket_layers
         self.device = next(model.parameters()).device
-        assert model.n_embd % 8 == 0, "flat parameter slots are 32-byte aligned; n_embd must be a multiple of 8"
-        self._handles = []
-        self._flatten()
-
-    # ------------------------------------------------------------------ flat storage
-    def _flatten(self):
-        m = self.m
-        order = [("emb", [m.tok_emb.weight, m.pos_emb, m.segm_emb.weight, m.texture_emb.weight, m.start_tok])]
-        for i, blk in enumerate(m.blocks):
+        m = model
+        C = m.n_embd
+        assert C % 8 == 0, "flat parameter slots are 32-byte aligned; n_embd must be a multiple of 8"
+        # backward-completion order; q | k | v and the 18 heads are groups, each read as one matrix
+        order = [tuple(m.head_list), m.ln_f]
+        for blk in reversed(list(m.blocks)):
             a = blk.attn
-            order.append((f"block{i}", [blk.ln1.weight, blk.ln1.bias, a.query.weight, a.key.weight, a.value.weight,
-                                        a.query.bias, a.key.bias, a.value.bias, a.proj.weight, a.proj.bias,
-                                        blk.ln2.weight, blk.ln2.bias, blk.mlp[0].weight, blk.mlp[0].bias,
-                                        blk.mlp[2].weight, blk.mlp[2].bias]))
-        order.append(("head", [m.ln_f.weight, m.ln_f.bias] + [h.weight for h in m.head_list]))
-        total, spans, self.group_span = 0, [], {}
-        for name, ps in order:
-            g0 = total
-            for p in ps:
-                n = (p.numel() + 7) // 8 * 8  # 32-byte aligned slots
-                spans.append((p, total, p.numel()))
-                total += n
-            self.group_span[name] = (g0, total)
-        dev = self.device
-        self.flat_p = torch.zeros(total, dtype=torch.float32, device=dev)
-        self.flat_g = torch.zeros(total, dtype=torch.float32, device=dev)
-        self.flat_m = torch.zeros(total, dtype=torch.float32, device=dev)
-        self.flat_v = torch.zeros(total, dtype=torch.float32, device=dev)
-        self.gview = {}
-        with torch.no_grad():
-            for p, off, n in spans:
-                self.flat_p[off:off + n].copy_(p.detach().reshape(-1))
-                p.data = self.flat_p[off:off + n].view_as(p)
-                gv = self.flat_g[off:off + n].view_as(p)
-                p.grad = gv
-                self.gview[id(p)] = gv
-        self.n_layers = len(m.blocks)
+            order += [blk.mlp[2], blk.mlp[0], blk.ln2, a.proj, (a.query, a.key, a.value), blk.ln1]
+        order += [m, m.tok_emb, m.segm_emb, m.texture_emb]     # m: its own pos_emb and start_tok
+        close = [m.ln_f] + [blk.ln1 for li, blk in enumerate(m.blocks) if li % bucket_layers == 0]
+        self.space = sp = ParamSpace(order, self.device, bucket_bytes=math.inf, close_after=close)
+        self.flat_p = sp.flat_p
+        self.heads = sp.joint([h.weight for h in m.head_list], C)                       # (W, dW) [18*1024, C]
+        self.qkv = [sp.joint([b.attn.query.weight, b.attn.key.weight, b.attn.value.weight], C) +
+                    sp.joint([b.attn.query.bias, b.attn.key.bias, b.attn.value.bias]) for b in m.blocks]  # W dW b db
         self.sync_from_rank0()
+
+    @property
+    def step_count(self):
+        return self.space.step_count
 
     def sync_from_rank0(self):
         """Replicas must start (and resume) from identical parameters and optimiser state -- torch DDP broadcasts
         them at construction; call this again after loading a checkpoint on one rank.  The random draws
         (``q_sample`` masks, diffusion times) should differ per rank: pass each rank its own ``generator``."""
-        if dist.is_initialized() and dist.get_world_size() > 1:
-            for t in (self.flat_p, self.flat_m, self.flat_v):
-                dist.broadcast(t, 0)
-            self._drop_packed_caches()
+        self.space.sync_from_rank0()
+        drop_packed_caches(self.m)
 
     def g(self, p):
-        return self.gview[id(p)]
-
-    def _flat_view(self, flat, p, rows, cols):
-        """[rows, cols] view of ``flat`` starting at parameter p's slot (spans adjacent parameters)"""
-        off = self.gview[id(p)].storage_offset()
-        return flat[off:off + rows * cols].view(rows, cols)
+        return self.space.g(p)
 
     def _weight_planes(self):
         """fp16 planes [T,1,out,in] of every GEMM weight for this step (one conversion launch each).  The forward
         uses them K-major (y = x W^T); the data-gradient GEMMs read the SAME planes MN-major (dX = dY W)."""
-        m = self.m
-        C, F4 = m.n_embd, 4 * m.n_embd
-
-        def planes(p, rows, cols):
-            return ops.f32_to_planes_rows(self._flat_view(self.flat_p, p, rows, cols)).unsqueeze(1)
+        def planes(w):
+            return ops.f32_to_planes_rows(w.detach()).unsqueeze(1)
 
         wp = []
-        for blk in m.blocks:
-            a = blk.attn
-            wp.append(dict(qkv=planes(a.query.weight, 3 * C, C), proj=planes(a.proj.weight, C, C),
-                           fc1=planes(blk.mlp[0].weight, F4, C), fc2=planes(blk.mlp[2].weight, C, F4)))
-        return wp, planes(m.head_list[0].weight, m.num_head * m.head_class_num, C)
-
-    def _drop_packed_caches(self):
-        # the inference mirrors cache packed weights keyed on torch's version counters, which the raw-pointer
-        # Adam kernel does not bump
-        for mod in self.m.modules():
-            mod.__dict__.pop("_t2h_cache", None)
-            mod.__dict__.pop("_t2h_graphs", None)   # captured sampler graphs bake in the packed-weight pointers
+        for blk, qkv in zip(self.m.blocks, self.qkv):
+            wp.append(dict(qkv=planes(qkv[0]), proj=planes(blk.attn.proj.weight), fc1=planes(blk.mlp[0].weight),
+                           fc2=planes(blk.mlp[2].weight)))
+        return wp, planes(self.heads[0])
 
     # ------------------------------------------------------------------ diffusion bookkeeping (torch RNG)
     def q_sample(self, x_0, t, generator=None):
@@ -139,11 +104,10 @@ class SamplerTrainer:
         x = ops.embed_sum(idx, segm, tex, m.tok_emb.weight.detach(), m.pos_emb.detach()[0],
                           m.segm_emb.weight.detach(), m.texture_emb.weight.detach())
         saved = []
-        for blk, w in zip(m.blocks, wp):
+        for blk, w, (_, _, bqkv, _) in zip(m.blocks, wp, self.qkv):
             a = blk.attn
             s = {"x_in": x}
             h1 = ops.layer_norm(x, blk.ln1.weight.detach(), blk.ln1.bias.detach(), blk.ln1.eps)
-            bqkv = self._flat_view(self.flat_p, a.query.bias, 1, 3 * C)[0]
             qkv = ops.linear(h1, w["qkv"], bqkv, planes_out=True)                      # [Tt, M, 3C]: q | k | v
             sc = ops.mha_scores(qkv[:, :, :C], B, T, nh, k=qkv[:, :, C:2 * C])
             p = ops.softmax_rows(sc, scale=1.0 / math.sqrt(C // nh))
@@ -171,8 +135,9 @@ class SamplerTrainer:
         M = B * T
         nh = m.blocks[0].attn.n_head
         scale = 1.0 / math.sqrt(C // nh)
-        self.flat_g.zero_()
-        self._handles = []
+        sp = self.space
+        sp.flat_g.zero_()
+        sp.arm(reduce)
         # Static loss scale (a power of two, undone inside the Adam kernel): the gradient operands of the
         # backward GEMMs are fp16 hi/lo planes, whose absolute resolution is 2^-24; scaling the loss so that
         # |dlogits| <= 256 keeps every gradient tensor well inside fp16's normal range.  The bound on the
@@ -206,7 +171,7 @@ class SamplerTrainer:
         # ---- heads + final LayerNorm
         NK = m.num_head * m.head_class_num
         dl = ops.f32_to_planes_rows(dlogits)                              # [Tt, M, NK]
-        self._wgrad(dl, hf, self._flat_view(self.flat_g, m.head_list[0].weight, NK, C))   # dW_heads = dlogits^T hf
+        self._wgrad(dl, hf, self.heads[1])                               # dW_heads [NK, C] = dlogits^T hf
         d_hf = ops.linear(dl, w_heads, w_kn=True)                        # [M, C] = dlogits W_heads
         del dlogits, dl
         dx = torch.zeros((M, C), dtype=torch.float32, device=x_0.device)  # running gradient of the stream
@@ -215,10 +180,10 @@ class SamplerTrainer:
         dxo = ops.layernorm_bwd_(dx, d_hf, x_last, m.ln_f.weight.detach(), self.g(m.ln_f.weight), self.g(m.ln_f.bias),
                                  m.ln_f.eps, accumulate=False, want_planes=True,
                                  colsum_out=self.g(m.blocks[-1].mlp[2].bias))
-        self._bucket_done("head", reduce)
+        sp.done(m.ln_f)
 
         # ---- blocks, last to first; dx is updated in place
-        for li in range(self.n_layers - 1, -1, -1):
+        for li in range(len(m.blocks) - 1, -1, -1):
             blk, s, w = m.blocks[li], saved[li], wp[li]
             a = blk.attn
             fc1, fc2 = blk.mlp[0], blk.mlp[2]
@@ -246,31 +211,25 @@ class SamplerTrainer:
                        v_tok=True)                                                    # dK = dS^T Q
             # fused q|k|v projection
             dqkv = ops.f32_to_planes_rows(d_qkv)
-            ops.colsum_(self._flat_view(self.flat_g, a.query.bias, 1, 3 * C)[0], d_qkv)
-            self._wgrad(dqkv, s["h1"], self._flat_view(self.flat_g, a.query.weight, 3 * C, C))
+            _, gwqkv, _, gbqkv = self.qkv[li]
+            ops.colsum_(gbqkv, d_qkv)
+            self._wgrad(dqkv, s["h1"], gwqkv)
             d_h1 = ops.linear(dqkv, w["qkv"], w_kn=True)                              # [M,C]
             dxo = ops.layernorm_bwd_(dx, d_h1, s["x_in"], blk.ln1.weight.detach(), self.g(blk.ln1.weight),
                                      self.g(blk.ln1.bias), blk.ln1.eps, accumulate=True, want_planes=li > 0,
                                      colsum_out=self.g(m.blocks[li - 1].mlp[2].bias) if li > 0 else None)
             # dx = d x_in = the gradient of the previous layer's output
             saved[li] = None
-            if li % self.bucket_layers == 0:
-                hi = min(self.n_layers, li + self.bucket_layers)
-                self._bucket_done((li, hi), reduce)
+            sp.done(blk.ln1)
 
         # ---- embeddings
         ops.embed_bwd_(self.g(m.tok_emb.weight), dx, x_t.reshape(-1).contiguous())
         ops.embed_bwd_(self.g(m.pos_emb).view(-1, C), dx, None, T)
         ops.embed_bwd_(self.g(m.segm_emb.weight), dx, segm.reshape(-1).contiguous())
         ops.embed_bwd_(self.g(m.texture_emb.weight), dx, tex.reshape(-1).contiguous())
-        self._bucket_done("emb", reduce)
-        self.wait_reduced()
+        sp.done(m.texture_emb)
+        sp.wait()
         return loss, vb_loss
-
-    def wait_reduced(self):
-        for h in self._handles:
-            h.wait()
-        self._handles = []
 
     @staticmethod
     def _wgrad(dy, x, out):
@@ -280,29 +239,11 @@ class SamplerTrainer:
         ks = ops.wgrad_k_split(dy.shape[2], x.shape[2], dy.shape[1]) if ops.SPLIT_K["wgrad"] else 0
         ops.wgrad(dy, x, out, k_split=ks)
 
-    def _bucket_done(self, which, reduce):
-        """gradients of a contiguous slice of the flat buffer are final: start their all-reduce (sum) now,
-        asynchronously, so it overlaps the rest of the backward pass"""
-        if not (reduce and dist.is_initialized() and dist.get_world_size() > 1):
-            return
-        if isinstance(which, tuple):
-            a = self.group_span[f"block{which[0]}"][0]
-            b = self.group_span[f"block{which[1] - 1}"][1]
-        else:
-            a, b = self.group_span[which]
-        self._handles.append(dist.all_reduce(self.flat_g[a:b], op=dist.ReduceOp.SUM, async_op=True))
-
     # ------------------------------------------------------------------ optimiser
     def adam_step(self):
         """torch.optim.Adam(lr, weight_decay=0) on the flat buffers; gradients averaged over ranks"""
-        p0 = self.m.tok_emb.weight
-        assert p0.data_ptr() == self.flat_p.data_ptr() + 4 * self.gview[id(p0)].storage_offset(), \
-            "the model's parameters no longer alias the trainer's flat buffer (model.to() / .half() after construction?)"
-        self.step_count += 1
-        world = dist.get_world_size() if dist.is_initialized() else 1
-        ops.adam_(self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.lr, self.betas[0], self.betas[1],
-                  self.eps, self.step_count, grad_scale=1.0 / (world * self.loss_scale))
-        self._drop_packed_caches()
+        self.space.adam(self.lr, self.betas, self.eps, 1.0 / (world_size() * self.loss_scale))
+        drop_packed_caches(self.m)
 
     def optimize_parameters(self, x_0, target_own, segm, tex, generator=None):
         """one reference training step: sample t ~ U{1..T}, loss, backward, all-reduce, Adam"""

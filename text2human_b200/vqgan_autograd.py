@@ -18,6 +18,7 @@ import torch.nn as nn
 from . import conv_grad as G
 from . import ops
 from . import vqgan_train as VT
+from .flat_params import ConvP
 
 
 # ----------------------------------------------------------------------------
@@ -48,7 +49,7 @@ class StandaloneSpace:
     def _make(self, mod):
         w = mod.weight
         co, ci, k, _ = w.shape
-        cp = VT.ConvP()
+        cp = ConvP()
         cp.mod, cp.k, cp.co, cp.ci, cp.co_p, cp.ci_p = mod, k, co, ci, G.pad8(co), G.pad8(ci)
         cp.w = G.oihw_to_master(w.detach())
         cp.wn, cp.wt = G.weight_planes(cp.w)
@@ -79,9 +80,12 @@ class StandaloneSpace:
             return cp.gb[:cp.co]
         return self.gbuf.get(id(p))
 
+    def done(self, mod):
+        """no gradient buckets: the gradients are handed to autograd"""
+
 
 class _Host:
-    """the ``tr`` interface the layers expect (space lookup, bucket notifications) over one StandaloneSpace"""
+    """the ``tr`` interface the layers expect (space lookup) over one StandaloneSpace"""
 
     def __init__(self, want_grads):
         self.space = StandaloneSpace(want_grads)
@@ -91,9 +95,6 @@ class _Host:
 
     def space_of_param(self, p):
         return self.space
-
-    def done(self, mod):
-        pass
 
 
 def _params_with_owner(module):

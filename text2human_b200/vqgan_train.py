@@ -13,11 +13,10 @@ weight planes with negated taps; four parity launches for the strided convs), we
 MN-major operands, pixel-patch contraction, split over the SMs with TMA reduce-add), and the AttnBlock products.
 The HBM-bound pieces are the kernels of csrc/gan.cu.
 
-Storage: all parameters live in one flat fp32 buffer per optimiser; conv weights are kept TAP-MAJOR
-``[K*K, Cout_p, Cin_p]`` (the layout the kernels' packed operands and the weight-gradient kernel's output share), the
-``nn.Parameter`` objects become OIHW *views* of it (state_dict keys / shapes unchanged).  Gradients are a second flat
-buffer (``p.grad`` are views), laid out in backward-completion order so that contiguous buckets can be all-reduced
-(NCCL, sum) while the rest of the backward pass is still running; Adam is one launch per optimiser.
+Storage: generator and discriminator each have a ``flat_params.ParamSpace``: parameters, gradients and Adam moments
+in flat fp32 buffers (conv weights tap-major, the ``nn.Parameter`` objects OIHW views of them), gradient buckets
+all-reduced while the rest of the backward pass runs (the layers report each finished module with ``done``), one
+Adam launch per optimiser.
 
 A micro-batch behaves exactly like one DDP rank of the reference: its own BatchNorm batch statistics in the
 discriminator, its own adaptive weight, its own DiffAugment draws; gradients of micro-batches and ranks are averaged.
@@ -25,143 +24,16 @@ discriminator, its own adaptive weight, its own DiffAugment draws; gradients of 
 import math
 
 import torch
-import torch.distributed as dist
-import torch.nn as nn
 
 from . import conv_grad as G
 from . import ops
+from .dist import world_size
+from .flat_params import ParamSpace, drop_packed_caches, load_checkpoint, save_checkpoint
 from .ops import CVT_PLAIN, CVT_S2D, CVT_UP2X
 from .vqgan_arch import AttnBlock, Decoder, Discriminator, Downsample, Encoder, ResnetBlock, Upsample
 
+NETS = ("encoder", "decoder", "quantize", "quant_conv", "post_quant_conv")    # the generator's nets, as checkpointed
 DS = 256.0      # extra scale of the (small) attention-score gradients inside AttnBlock, undone by the consumer's alpha
-
-
-# ----------------------------------------------------------------------------
-# flat parameter storage
-# ----------------------------------------------------------------------------
-class ConvP:
-    """one conv layer's views into the flat buffers"""
-    __slots__ = ("mod", "k", "co", "ci", "co_p", "ci_p", "w", "gw", "b", "gb", "wn", "wt")
-
-
-class ParamSpace:
-    """Flat fp32 parameter / gradient / Adam-moment buffers for an ordered list of leaf modules.
-    ``order``: modules (Conv2d, GroupNorm, BatchNorm2d, Embedding) in backward-completion order."""
-
-    def __init__(self, order, device, bucket_bytes=48 << 20):
-        self.device = device
-        self.convs = {}
-        self.slots = []          # (param, offset, numel, master_shape or None)
-        total = 0
-
-        def take(n):
-            nonlocal total
-            off = total
-            total += (n + 7) // 8 * 8
-            return off
-
-        self.mod_span = []
-
-        def conv_slots(mods):
-            """weights of all ``mods`` first, then their biases (a fused q|k|v projection reads them as one matrix)"""
-            cps = []
-            for mod in mods:
-                co, ci, kh, kw = mod.weight.shape
-                assert kh == kw
-                cp = ConvP()
-                cp.mod, cp.k, cp.co, cp.ci, cp.co_p, cp.ci_p = mod, kh, co, ci, G.pad8(co), G.pad8(ci)
-                self.slots.append((mod.weight, take(kh * kw * cp.co_p * cp.ci_p), None, cp))
-                self.convs[mod] = cp
-                cps.append(cp)
-            for mod, cp in zip(mods, cps):
-                if mod.bias is not None:
-                    self.slots.append((mod.bias, take(cp.co_p), None, ("bias", cp)))
-
-        for mod in order:
-            start = total
-            if isinstance(mod, tuple):           # fused group of convs
-                conv_slots(mod)
-                for m_ in mod[:-1]:
-                    self.mod_span.append((m_, start, start))   # empty spans: the group closes with its last member
-                self.mod_span.append((mod[-1], start, total))
-                continue
-            if isinstance(mod, nn.Conv2d):
-                conv_slots((mod,))
-            else:
-                for p in mod.parameters(recurse=False):
-                    self.slots.append((p, take(p.numel()), None, None))
-            self.mod_span.append((mod, start, total))
-        self.total = total
-        self.flat_p = torch.zeros(total, dtype=torch.float32, device=device)
-        self.flat_g = torch.zeros(total, dtype=torch.float32, device=device)
-        self.flat_m = torch.zeros(total, dtype=torch.float32, device=device)
-        self.flat_v = torch.zeros(total, dtype=torch.float32, device=device)
-        self.gview = {}
-        with torch.no_grad():
-            for p, off, _, tag in self.slots:
-                if isinstance(tag, ConvP):
-                    cp = tag
-                    n = cp.k * cp.k * cp.co_p * cp.ci_p
-                    m = self.flat_p[off:off + n].view(cp.k * cp.k, cp.co_p, cp.ci_p)
-                    m.copy_(G.oihw_to_master(p.detach().to(device)))
-                    cp.w = m
-                    cp.gw = self.flat_g[off:off + n].view(cp.k * cp.k, cp.co_p, cp.ci_p)
-                    p.data = G.master_as_oihw(m, cp.co, cp.ci, cp.k)
-                    p.grad = G.master_as_oihw(cp.gw, cp.co, cp.ci, cp.k)
-                    cp.b = cp.gb = None
-                elif isinstance(tag, tuple):
-                    cp = tag[1]
-                    self.flat_p[off:off + cp.co].copy_(p.detach().reshape(-1))
-                    cp.b = self.flat_p[off:off + cp.co_p]
-                    cp.gb = self.flat_g[off:off + cp.co_p]
-                    p.data = self.flat_p[off:off + cp.co]
-                    p.grad = self.flat_g[off:off + cp.co]
-                else:
-                    n = p.numel()
-                    self.flat_p[off:off + n].copy_(p.detach().reshape(-1))
-                    p.data = self.flat_p[off:off + n].view_as(p)
-                    p.grad = self.flat_g[off:off + n].view_as(p)
-                self.gview[id(p)] = p.grad
-        # gradient buckets: contiguous runs of whole modules, in backward-completion order
-        self.buckets, self.bucket_last = [], {}
-        b0 = 0
-        for i, (mod, s, e) in enumerate(self.mod_span):
-            if (e - b0) * 4 >= bucket_bytes or i == len(self.mod_span) - 1:
-                self.bucket_last[mod] = len(self.buckets)
-                self.buckets.append((b0, e))
-                b0 = e
-        self.step_count = 0
-
-    def g(self, p):
-        return self.gview[id(p)]
-
-    def prepare(self, terms):
-        """fp16 planes of every conv weight for this step: forward operand wn and transposed (data-gradient) wt"""
-        for cp in self.convs.values():
-            cp.wn, cp.wt = G.weight_planes(cp.w, terms)
-
-    def release(self):
-        for cp in self.convs.values():
-            cp.wn = cp.wt = None
-
-    def adam(self, lr, betas, eps, grad_scale):
-        self.step_count += 1
-        ops.adam_(self.flat_p, self.flat_g, self.flat_m, self.flat_v, lr, betas[0], betas[1], eps, self.step_count,
-                  grad_scale=grad_scale)
-
-    def sync_from_rank0(self):
-        """replicas start (and resume) from identical parameters and optimiser state, as torch DDP guarantees"""
-        if dist.is_initialized() and dist.get_world_size() > 1:
-            for t in (self.flat_p, self.flat_m, self.flat_v):
-                dist.broadcast(t, 0)
-
-    def state(self):
-        return dict(flat_m=self.flat_m.clone(), flat_v=self.flat_v.clone(), step=self.step_count)
-
-    def load_state(self, st):
-        self.flat_m.copy_(st["flat_m"])
-        self.flat_v.copy_(st["flat_v"])
-        self.step_count = int(st["step"])
 
 
 # ----------------------------------------------------------------------------
@@ -204,6 +76,9 @@ class Layer:
     def gof(self, p):
         return self.tr.space_of_param(p).g(p)
 
+    def done(self, mod):
+        self.tr.space_of(mod).done(mod)
+
     def bias_grad(self, cp, g):
         """cp.gb += column sums of the output gradient ``g`` (a Grad, or a bare fp32 NHWC tensor)"""
         if cp.gb is None:
@@ -244,7 +119,7 @@ class ConvL(Layer):
         dyp = grad.planes()
         self.bias_grad(cp, grad)
         G.wgrad(self.kind, dyp, a, cp.gw, n=N)
-        self.tr.done(self.conv)
+        self.done(self.conv)
         if not self.need_dx:
             return None
         dx = G.dgrad(self.kind, dyp, cp.wt, n=N, in_hw=(H, W))
@@ -273,7 +148,7 @@ class ConvInImageL(Layer):
         cp = self.cp(self.conv)
         self.bias_grad(cp, grad)
         G.wgrad("k3", grad.planes(), a, cp.gw, n=N)
-        self.tr.done(self.conv)
+        self.done(self.conv)
         return None
 
 
@@ -344,7 +219,7 @@ class NormConvOutL(Layer):
             cp.gw.add_(gw_known)
         else:
             G.wgrad("k3", dyp, a, cp.gw, n=N)
-        self.tr.done(self.conv)
+        self.done(self.conv)
         # pass 1 of the norm backward (sum du, sum du*xhat) rides in the data-gradient conv's epilogue where it can
         nb = ops.nb_context(x, st, self.norm.weight.detach(), self.norm.bias.detach(), act="swish", groups=32,
                             eps=self.norm.eps)
@@ -353,7 +228,7 @@ class NormConvOutL(Layer):
         dx, dxp = ops.norm_bwd(x, st, self.norm.weight.detach(), self.norm.bias.detach(), da, act="swish", groups=32,
                                eps=self.norm.eps, dgamma=self.gof(self.norm.weight), dbeta=self.gof(self.norm.bias),
                                want_planes=True, colsum_out=cs, sums=nb["sums"] if nb else None)
-        self.tr.done(self.norm)
+        self.done(self.norm)
         return Grad(dx, dxp, cs)
 
 
@@ -393,7 +268,7 @@ class ResL(Layer):
         dop = grad.planes()
         self.bias_grad(c2, grad)
         G.wgrad("k3", dop, a2, c2.gw, n=N)
-        self.tr.done(b.conv2)
+        self.done(b.conv2)
         nb2 = ops.nb_context(h1, st2, b.norm2.weight.detach(), b.norm2.bias.detach(), act="swish", groups=32,
                              eps=b.norm2.eps)
         d_a2 = G.dgrad("k3", dop, c2.wt, n=N, in_hw=(H, W), nb=nb2)
@@ -402,10 +277,10 @@ class ResL(Layer):
                                    dbeta=self.gof(b.norm2.bias), want_planes=True, want_dx=False,
                                    colsum_out=c1.gb[:h1.shape[-1]] if c1.gb is not None else None,   # conv1's bias gradient
                                    sums=nb2["sums"] if nb2 else None)
-        self.tr.done(b.norm2)
+        self.done(b.norm2)
         del d_a2, a2, h1
         G.wgrad("k3", d_h1p, a1, c1.gw, n=N)
-        self.tr.done(b.conv1)
+        self.done(b.conv1)
         nb1 = ops.nb_context(x, st1, b.norm1.weight.detach(), b.norm1.bias.detach(), act="swish", groups=32,
                              eps=b.norm1.eps)
         d_a1 = G.dgrad("k3", d_h1p, c1.wt, n=N, in_hw=(H, W), nb=nb1)
@@ -415,13 +290,13 @@ class ResL(Layer):
             cs = self.cp(b.nin_shortcut)
             self.bias_grad(cs, grad)
             G.wgrad("k1", dop, xp, cs.gw, n=N)
-            self.tr.done(b.nin_shortcut)
+            self.done(b.nin_shortcut)
             d_sc = G.dgrad("k1", dop, cs.wt, n=N, in_hw=(H, W))
         csum = torch.zeros(x.shape[-1], dtype=torch.float32, device=x.device)
         dx, dxp = ops.norm_bwd(x, st1, b.norm1.weight.detach(), b.norm1.bias.detach(), d_a1, act="swish", groups=32,
                                eps=b.norm1.eps, dgamma=self.gof(b.norm1.weight), dbeta=self.gof(b.norm1.bias),
                                add=d_sc, want_planes=True, colsum_out=csum, sums=nb1["sums"] if nb1 else None)
-        self.tr.done(b.norm1)
+        self.done(b.norm1)
         return Grad(dx, dxp, csum)
 
 
@@ -437,19 +312,14 @@ class AttnL(Layer):
         """-> (W [3C, C], dW, b [3C], db): q | k | v as one projection.  In the trainer's flat space the three
         weights (and biases) are adjacent, so these are views; a space with separate per-conv buffers gets one
         concatenated copy whose slices REPLACE the per-conv buffers (gradients then land where grad_of looks)."""
-        q, k, v = (self.cp(m) for m in (self.b.q, self.b.k, self.b.v))
+        mods = (self.b.q, self.b.k, self.b.v)
+        q, k, v = (self.cp(m) for m in mods)
         Cc = q.co
         sp = self.tr.space_of(self.b.q)
-        if hasattr(sp, "flat_p"):
-            off_w = q.w.storage_offset()
-            off_b = q.b.storage_offset()
-            assert k.w.storage_offset() == off_w + Cc * Cc and v.w.storage_offset() == off_w + 2 * Cc * Cc
-            assert k.b.storage_offset() == off_b + Cc and v.b.storage_offset() == off_b + 2 * Cc
-
-            def view(flat, off, r, c):
-                return flat[off:off + r * c].view(r, c)
-            return (view(sp.flat_p, off_w, 3 * Cc, Cc), view(sp.flat_g, off_w, 3 * Cc, Cc),
-                    sp.flat_p[off_b:off_b + 3 * Cc], sp.flat_g[off_b:off_b + 3 * Cc])
+        if isinstance(sp, ParamSpace):
+            w, gw = sp.joint([m.weight for m in mods], Cc)
+            b, gb = sp.joint([m.bias for m in mods])
+            return w, gw, b, gb
         hit = getattr(self, "_qkv_cat", None)
         if hit is None:
             w = torch.cat([c_.w[0] for c_ in (q, k, v)], 0).contiguous()
@@ -492,7 +362,7 @@ class AttnL(Layer):
         dop = grad.planes().view(T, M, Cc)
         self.bias_grad(cpo, grad)
         ops.wgrad(dop, o, cpo.gw[0], k_split=ops.wgrad_k_split(Cc, Cc, M), accumulate=True)
-        self.tr.done(b.proj_out)
+        self.done(b.proj_out)
         d_o = ops.linear(dop, cpo.wn, w_kn=True, planes_out=True)                       # planes [T,M,C] = dY Wp
         q, k, v = qkv[:, :, :Cc], qkv[:, :, Cc:2 * Cc], qkv[:, :, 2 * Cc:]
         d_qkv = torch.empty((M, 3 * Cc), dtype=torch.float32, device=x.device)
@@ -507,13 +377,13 @@ class AttnL(Layer):
         ops.colsum_(gbqkv, d_qkv)
         ops.wgrad(dqkvp, hn.view(T, M, Cc), gwqkv, k_split=ops.wgrad_k_split(3 * Cc, Cc, M), accumulate=True)
         for m_ in (b.q, b.k, b.v):
-            self.tr.done(m_)
+            self.done(m_)
         d_hn = ops.linear(dqkvp, wp, w_kn=True)                                         # [M, C]
         csum = torch.zeros(Cc, dtype=torch.float32, device=x.device)
         dx, dxp = ops.norm_bwd(x, st, b.norm.weight.detach(), b.norm.bias.detach(), d_hn.view(N, H, W, Cc), act=None,
                                groups=32, eps=b.norm.eps, dgamma=self.gof(b.norm.weight),
                                dbeta=self.gof(b.norm.bias), add=grad.g, want_planes=True, colsum_out=csum)
-        self.tr.done(b.norm)
+        self.done(b.norm)
         return Grad(dx, dxp, csum)
 
 
@@ -538,7 +408,7 @@ class Lin1x1L(Layer):
         dyp = grad.planes()
         self.bias_grad(cp, grad)
         G.wgrad("k1", dyp, a, cp.gw, n=N)
-        self.tr.done(self.conv)
+        self.done(self.conv)
         return Grad(G.dgrad("k1", dyp, cp.wt, n=N, in_hw=(H, W)))
 
 
@@ -684,7 +554,7 @@ class DiscNet(Layer):
         if want_params:
             ops.colsum_(cl.gb[:1], dlogits.reshape(-1, 1))
             G.wgrad("k4s1", dlp, h, cl.gw, n=N)
-            self.tr.done(self.last)
+            self.done(self.last)
         g = G.dgrad("k4s1", dlp, cl.wt, n=N, in_hw=(hh, ww))
         for conv, bn, kind in reversed(self.mid):
             a, pre, st, hh, ww = rec.pop()
@@ -695,9 +565,9 @@ class DiscNet(Layer):
                                        dbeta=self.gof(bn.bias) if want_params else None, want_planes=True, n=1,
                                        want_dx=False)
             if want_params:
-                self.tr.done(bn)
+                self.done(bn)
                 G.wgrad(kind, dprep, a, cp.gw, n=N)
-                self.tr.done(conv)
+                self.done(conv)
             g = G.dgrad(kind, dprep, cp.wt, n=N, in_hw=(hh, ww))
         a0, y0, H, W = rec.pop()
         c0 = self.cp(self.first)
@@ -705,7 +575,7 @@ class DiscNet(Layer):
         if want_params:
             self.bias_grad(c0, dpre)
             G.wgrad("k4s2", dprep, a0, c0.gw, n=N)
-            self.tr.done(self.first)
+            self.done(self.first)
         if want_input:
             G.dgrad("k4s2", dprep, c0.wt, n=N, in_hw=(H, W), cin=3, out=dx_out, d_strides=(3 * H * W, W, 1, H * W))
         return dx_out
@@ -739,20 +609,16 @@ class VQGANTrainer:
                 self._space[mod] = sp
         self._pspace = {}
         for sp in (self.gen, self.dsc):
-            for p, _, _, _ in sp.slots:
+            for p, _, _ in sp.slots:
                 self._pspace[id(p)] = sp
-        ws = model.quantize.embedding_list
-        off = self.gen.g(ws[0].weight).storage_offset()
-        n_e, D = ws[0].weight.shape
-        self.codebook = self.gen.flat_p[off:off + 18 * n_e * D].view(18, n_e, D)
-        self.g_codebook = self.gen.flat_g[off:off + 18 * n_e * D].view(18, n_e, D)
-        assert self.gen.g(ws[17].weight).storage_offset() == off + 17 * n_e * D
-        self._handles = []
-        self._reduce = False
+        ws = [e.weight for e in model.quantize.embedding_list]
+        n_e, D = ws[0].shape
+        cb, gcb = self.gen.joint(ws, D)
+        self.codebook, self.g_codebook = cb.view(18, n_e, D), gcb.view(18, n_e, D)
+        self.force_no_reduce = False    # True: no gradient all-reduce even with several ranks
         self.aug_draw_fn = None     # tests inject the reference's recorded DiffAugment draws here
         self.log = {}
-        self.gen.sync_from_rank0()
-        self.dsc.sync_from_rank0()
+        self._sync_from_rank0()
 
     # ---- plumbing used by the layers
     def space_of(self, mod):
@@ -761,28 +627,14 @@ class VQGANTrainer:
     def space_of_param(self, p):
         return self._pspace[id(p)]
 
-    def done(self, mod):
-        """all gradients of ``mod`` are final for this step: if it closes a bucket, start that bucket's all-reduce
-        (asynchronously, on NCCL's stream) while the backward pass continues"""
-        if not self._reduce:
-            return
-        sp = self._space[mod]
-        b = sp.bucket_last.get(mod)
-        if b is not None and self._armed.get((id(sp), b), False):
-            a, e = sp.buckets[b]
-            self._handles.append(dist.all_reduce(sp.flat_g[a:e], op=dist.ReduceOp.SUM, async_op=True))
-            self._armed[(id(sp), b)] = False
-
-    def _arm(self, sp, on):
-        """buckets fire only during the LAST micro-batch's backward of that parameter space"""
-        self._reduce = (on and dist.is_initialized() and dist.get_world_size() > 1 and
-                        not getattr(self, "force_no_reduce", False))
-        self._armed = {(id(sp), b): True for b in range(len(sp.buckets))} if self._reduce else {}
-
     def wait_reduced(self):
-        for h in self._handles:
-            h.wait()
-        self._handles = []
+        self.gen.wait()
+        self.dsc.wait()
+
+    def _sync_from_rank0(self):
+        self.gen.sync_from_rank0()
+        self.dsc.sync_from_rank0()
+        drop_packed_caches(self.model, self.disc)
 
     # ---- random draws of DiffAugment, in the reference's order (vqgan_loss.py:47-79)
     def _aug_draws(self, B, H, W, device, generator=None):
@@ -821,7 +673,7 @@ class VQGANTrainer:
         dz = ops.vq_bwd(z, self.codebook, idx, ids, g.g, self.g_codebook, 2.0 * cb_scale / nel,
                         2.0 * self.beta * cb_scale / nel)
         for e in self.model.quantize.embedding_list:
-            self.done(e)
+            self.gen.done(e)
         g = self.qconv.bwd(Grad(dz))
         self.enc_in.bwd(self.enc_body.bwd(self.enc_out.bwd(g.g)))
         self._vq = None
@@ -831,6 +683,7 @@ class VQGANTrainer:
         B, _, H, W = x.shape
         dev = x.device
         S = self.loss_scale
+        reduce = last and not self.force_no_reduce      # buckets fire during the LAST micro-batch's backward only
         acc = torch.zeros(8, dtype=torch.float64, device=dev)   # l1 sum, fake-logit sum, sqerr, hinge real, hinge fake
         dw = torch.zeros(1, dtype=torch.float32, device=dev)
         xrec, sqerr, z_numel = self.gen_forward(x, mask)
@@ -850,10 +703,9 @@ class VQGANTrainer:
         rg, gg = self.dec_out.wgrad_pair(g_nll, g_g)
         ops.adaptive_weight(rg, gg, dw, 1.0 / S, self.disc_weight_max, 1.0 if step >= self.disc_start_step else 0.0)
         dxrec = ops.axpy_dev(g_nll, g_g, dw)                 # loss = nll + d_weight * g_loss + codebook_loss
-        self._arm(self.gen, last)
+        self.gen.arm(reduce)
         # conv_out's weight gradient is linear in dxrec: rg + d_weight * gg, no third weight-gradient launch
         self.gen_backward(dxrec, S, conv_out_gw=ops.axpy_dev(rg, gg, dw))
-        self._reduce = False
         out = dict(acc=acc, dw=dw, nel=nel, n_logit=logits_fake.numel(), sqerr=sqerr, z_numel=z_numel)
         # ---- discriminator update (step > disc_start_step, vqgan_model.py:475-486)
         if step > self.disc_start_step:
@@ -867,11 +719,10 @@ class VQGANTrainer:
             lf_ = self.dnet.fwd(xr)
             d_lr = ops.hinge_loss(lr_, acc[3:4], 1.0, gscale=0.5 * Sd / lr_.numel())
             d_lf2 = ops.hinge_loss(lf_, acc[4:5], -1.0, gscale=0.5 * Sd / lf_.numel())
-            self._arm(self.dsc, False)
+            self.dsc.arm(False)
             self.dnet.bwd(d_lf2, want_params=True, want_input=False)
-            self._arm(self.dsc, last)
+            self.dsc.arm(reduce)
             self.dnet.bwd(d_lr, want_params=True, want_input=False)
-            self._reduce = False
             out["n_dlogit"] = lr_.numel()
         return out
 
@@ -892,7 +743,6 @@ class VQGANTrainer:
         self.n_micro = n_micro
         self.gen.flat_g.zero_()
         self.dsc.flat_g.zero_()
-        self._handles = []
         self.gen.prepare(terms)
         self.dsc.prepare(terms)
         outs = []
@@ -919,36 +769,27 @@ class VQGANTrainer:
         return out
 
     def adam_step(self):
-        world = dist.get_world_size() if dist.is_initialized() else 1
+        world = world_size()
         self.wait_reduced()
         self.gen.adam(self.lr, self.betas, self.eps, 1.0 / (world * self.n_micro * self.loss_scale))
         if self._did_disc:
             self.dsc.adam(self.lr, self.betas, self.eps, 1.0 / (world * self.n_micro * self.disc_scale))
-        for mod in list(self.model.modules()) + list(self.disc.modules()):
-            mod.__dict__.pop("_t2h_cache", None)
+        drop_packed_caches(self.model, self.disc)
 
     def optimize_parameters(self, data, step, generator=None):
         self.training_step(data, step, generator)
         self.adam_step()
 
     # ---- checkpoint / resume incl. optimiser state (the reference saves only the networks, vqgan_model.py:59-84)
+    def _nets(self):
+        return dict({k: getattr(self.model, k) for k in NETS}, discriminator=self.disc)
+
     def save(self, path):
-        m = self.model
-        net = {k: {kk: vv.detach().clone().contiguous() for kk, vv in getattr(m, k).state_dict().items()}
-               for k in ("encoder", "decoder", "quantize", "quant_conv", "post_quant_conv")}
-        net["discriminator"] = {k: v.detach().clone().contiguous() for k, v in self.disc.state_dict().items()}
-        torch.save(dict(net, optimizer=dict(gen=self.gen.state(), disc=self.dsc.state())), path)
+        save_checkpoint(path, self._nets(), dict(gen=self.gen.state(), disc=self.dsc.state()))
 
     def load(self, path):
-        ck = torch.load(path, map_location=self.device)
-        m = self.model
-        for k in ("encoder", "decoder", "quantize", "quant_conv", "post_quant_conv"):
-            getattr(m, k).load_state_dict(ck[k], strict=True)
-        self.disc.load_state_dict(ck["discriminator"], strict=True)
-        if "optimizer" in ck:
-            self.gen.load_state(ck["optimizer"]["gen"])
-            self.dsc.load_state(ck["optimizer"]["disc"])
-        for mod in list(m.modules()) + list(self.disc.modules()):
-            mod.__dict__.pop("_t2h_cache", None)
-        self.gen.sync_from_rank0()
-        self.dsc.sync_from_rank0()
+        opt = load_checkpoint(path, self._nets(), self.device)
+        if opt is not None:
+            self.gen.load_state(opt["gen"])
+            self.dsc.load_state(opt["disc"])
+        self._sync_from_rank0()
