@@ -410,9 +410,9 @@ int t2h_conv_wgrad(const t2h_conv_wgrad_params* p, t2h_stream_t stream);
 /* Backward of y = act(norm(x)*gamma + beta) for GroupNorm(groups) per image (Normalize(), vqgan_arch.py:510) or,
  * with n = 1 / hw = N*H*W / groups = c, training-mode BatchNorm2d.  stats as t2h_gn_stats / the conv epilogue
  * produced them.  dx = add (optional) + dL/dx as fp32 and / or fp16 planes (either may be NULL, not both: a
- * gradient only the following conv gradients consume needs no fp32 copy); dgamma/dbeta accumulated (may be NULL).
- * ws: 2*n*c doubles of scratch.  act: 0 none, 1 swish, 2 LeakyReLU(0.2).  dx_colsum (optional, [c], accumulated):
- * column sums of the dx written = the bias gradient of the conv whose output x is.  sums_ready != 0: ws already
+ * gradient only the following conv gradients consume needs no fp32 copy); dgamma/dbeta accumulated (each may be
+ * NULL, independently of the other).  c % 4 == 0, c <= 2048.  ws: 2*n*c doubles of scratch.  act: 0 none,
+ * 1 swish, 2 LeakyReLU(0.2).  dx_colsum (optional, [c], accumulated): column sums of the dx written = the bias gradient of the conv whose output x is.  sums_ready != 0: ws already
  * holds pass 1's per-(image, channel) sums {sum du, sum du*xhat} -- the data-gradient conv that produced dy
  * accumulated them in its epilogue (t2h_tapgemm_params.nb_sums) -- and only the apply pass runs. */
 int t2h_norm_bwd(const float* x, const double* stats, const float* gamma, const float* beta, const float* dy,

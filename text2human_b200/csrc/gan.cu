@@ -123,7 +123,8 @@ __global__ void norm_bwd_apply_kernel(const float* __restrict__ x, const double*
   const long long work = (long long)min((long long)pix_per_block, HW - p_begin) * c4;
   const long long base = ((long long)n * HW + p_begin) * C;
   // column sums of the dx written (= the bias gradient of the conv that produced x): when blockDim is a multiple of
-  // C/4 a thread always meets the same 4 channels and keeps them in registers
+  // C/4 a thread always meets the same 4 channels and keeps them in registers, otherwise it adds each element to
+  // the block's shared column sums (tests/test_gpu_backward_paths.py::norm_bwd_route restates this choice)
   const bool fixed_cols = (blockDim.x % c4) == 0;
   float cs[4] = {0.f, 0.f, 0.f, 0.f};
   for (long long i = threadIdx.x; i < work; i += blockDim.x) {
@@ -184,8 +185,8 @@ __global__ void norm_bwd_params_kernel(const double* __restrict__ S, float* __re
     a += S[((long long)n * C + c) * 2 + 0];
     b += S[((long long)n * C + c) * 2 + 1];
   }
-  dbeta[c] += (float)a;
-  dgamma[c] += (float)b;
+  if (dbeta) dbeta[c] += (float)a;
+  if (dgamma) dgamma[c] += (float)b;
 }
 
 // BatchNorm running statistics (momentum update with the unbiased batch variance), stats = (sum, sumsq) per channel
@@ -569,6 +570,21 @@ __global__ void sample_step_kernel(const float* __restrict__ logits, const float
   }
 }
 
+// t2h_norm_bwd's kernels keep per-channel constants in dynamic shared memory: 6 C floats (reduce) and 7 C floats
+// (apply), 56 KB at the largest C.  Above the default 48 KB a kernel must be opted in, once per device (the
+// attribute lives in the device's copy of the function); model shapes stay below it and never call this.
+constexpr int kNormBwdMaxC = 2048;
+static int smem_opt_in(const void* kernel, size_t bytes, int max_bytes, bool (&configured)[64]) {
+  if (bytes <= 48 * 1024) return T2H_OK;
+  int dev = 0;
+  T2H_CUDA(cudaGetDevice(&dev));
+  if (!configured[dev & 63]) {
+    T2H_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_bytes));
+    configured[dev & 63] = true;
+  }
+  return T2H_OK;
+}
+
 }  // namespace t2h
 
 using namespace t2h;
@@ -580,35 +596,47 @@ int t2h_norm_bwd(const float* x, const double* stats, const float* gamma, const 
                  int n, int hw, int c, int groups, float eps, int act, float* dx_colsum, int sums_ready,
                  t2h_stream_t stream) {
   T2H_CHECK_ARG(x && stats && gamma && beta && dy && (dx || dx_planes) && ws && n > 0 && hw > 0, "norm_bwd: bad args");
-  T2H_CHECK_ARG(c % groups == 0 && c % 4 == 0 && c <= 2048, "norm_bwd: C=%d groups=%d unsupported", c, groups);
+  T2H_CHECK_ARG(c % groups == 0 && c % 4 == 0 && c <= kNormBwdMaxC, "norm_bwd: C=%d groups=%d unsupported", c,
+                groups);
   T2H_CHECK_ARG(act >= 0 && act <= 2 && (terms == 1 || terms == 2 || !dx_planes), "norm_bwd: act=%d terms=%d", act,
                 terms);
   cudaStream_t st = as_stream(stream);
+  // (tests/test_gpu_backward_paths.py::norm_bwd_route restates the block, lane and pixels-per-block choices below)
   if (!sums_ready) {  // pass 1 (skipped when the conv that produced dy accumulated the sums in its epilogue)
     T2H_CUDA(cudaMemsetAsync(ws, 0, sizeof(double) * 2 * (size_t)n * c, st));
     const int c4 = c / 4;
     int block = 256;
     if (c4 > block) block = ((c4 + 31) / 32) * 32;
     T2H_CHECK_ARG(block <= 1024, "norm_bwd: C=%d too large", c);
-    block = (block / c4) * c4;
+    block = (block / c4) * c4;  // C > 1024: block = C/4, one pixel lane
     const int lanes = block / c4;
     int blocks_x = ceil_div(num_sms() * 4, n);
     int ppb = ceil_div(hw, blocks_x);
     if (ppb < lanes * 8) ppb = lanes * 8;
     blocks_x = ceil_div(hw, ppb);
-    norm_bwd_reduce_kernel<<<dim3(blocks_x, n), block, 6 * c * sizeof(float), st>>>(x, stats, gamma, beta, dy, ws,
-                                                                                 hw, c, groups, eps, act, ppb);
+    static bool reduce_configured[64] = {};
+    const size_t smem = 6 * (size_t)c * sizeof(float);
+    int rc = smem_opt_in((const void*)norm_bwd_reduce_kernel, smem, 6 * kNormBwdMaxC * (int)sizeof(float),
+                         reduce_configured);
+    if (rc) return rc;
+    norm_bwd_reduce_kernel<<<dim3(blocks_x, n), block, smem, st>>>(x, stats, gamma, beta, dy, ws, hw, c, groups, eps,
+                                                                   act, ppb);
     T2H_LAUNCH_OK();
   }
   int bx2 = ceil_div(num_sms() * 8, n);
   int ppb2 = ceil_div(hw, bx2);
   if (ppb2 < 16) ppb2 = 16;
   bx2 = ceil_div(hw, ppb2);
-  norm_bwd_apply_kernel<<<dim3(bx2, n), 256, 7 * c * sizeof(float), st>>>(
+  static bool apply_configured[64] = {};
+  const size_t smem2 = 7 * (size_t)c * sizeof(float);
+  int rc = smem_opt_in((const void*)norm_bwd_apply_kernel, smem2, 7 * kNormBwdMaxC * (int)sizeof(float),
+                       apply_configured);
+  if (rc) return rc;
+  norm_bwd_apply_kernel<<<dim3(bx2, n), 256, smem2, st>>>(
       x, stats, gamma, beta, dy, ws, add, dx, reinterpret_cast<__half*>(dx_planes), terms, (long long)n * hw * c, hw,
       c, groups, eps, act, ppb2, dx_colsum);
   T2H_LAUNCH_OK();
-  if (dgamma && dbeta) {
+  if (dgamma || dbeta) {  // either may be given alone
     norm_bwd_params_kernel<<<ceil_div(c, 128), 128, 0, st>>>(ws, dgamma, dbeta, n, c);
     T2H_LAUNCH_OK();
   }

@@ -1107,6 +1107,7 @@ extern "C" int t2h_conv_wgrad(const t2h_conv_wgrad_params* p, t2h_stream_t strea
                 (long long)p->dw_ld);
   TapGemmDev P;
   memset(&P, 0, sizeof(P));
+  // (tests/test_gpu_backward_paths.py::wgrad_route restates the patch shape, BN, column tiles and split-K below)
   int PW = 16;
   while (PW > 1 && PW / 2 >= p->W) PW >>= 1;  // narrow images: taller patches
   const int PH = 64 / PW;
