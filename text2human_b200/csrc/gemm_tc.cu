@@ -802,6 +802,7 @@ static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensor
   return T2H_OK;
 }
 
+template <bool kPair>
 static int launch_swap(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
                        const CUtensorMap& tmR, const TapGemmDev& P, cudaStream_t stream) {
   using C = Cfg<128>;
@@ -809,19 +810,23 @@ static int launch_swap(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   int dev = 0;
   T2H_CUDA(cudaGetDevice(&dev));
   if (!configured[dev & 63]) {
-    T2H_CUDA(cudaFuncSetAttribute(tapgemm_swap_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDynSmem));
+    T2H_CUDA(cudaFuncSetAttribute(tapgemm_swap_kernel<kPair>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  kDynSmem));
     configured[dev & 63] = true;
   }
   TapGemmDev Q = P;
-  // ring depths from what the register epilogue leaves of the shared memory: 4 A slabs load the next chunk's hi and
-  // lo slabs during the whole current chunk, the rest holds weight tiles (4: two taps of the 3-product order ahead).
+  // ring depths from what the register epilogue leaves of the shared memory.  Unpaired: 4 A slabs load the next
+  // chunk's hi and lo slabs during the whole current chunk, the rest holds weight tiles (4: two taps of the 3-product
+  // order ahead).  Paired: each slot feeds twice the MMA work, 3 pair slabs + 3 weight tiles.
   // The kernel's ring invariant needs a_slots >= 2 and b_slots >= 2.
-  Q.a_slots = 4;
-  int nb = (kSwapRingBytes - Q.a_slots * C::kASlot) / C::kBSlot;
+  const int a_slot = kPair ? kSwapPairASlot : C::kASlot;
+  Q.a_slots = kPair ? 3 : 4;
+  int nb = (kSwapRingBytes - Q.a_slots * a_slot) / C::kBSlot;
   Q.b_slots = nb > kMaxSlots ? kMaxSlots : nb;
   if (Q.b_slots < 2) return fail(T2H_EINVAL, "tapgemm: shared-memory rings do not fit");
   int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
-  T2H_CUDA(launch_pdl(tapgemm_swap_kernel, dim3(grid), dim3(kSwapThreads), kDynSmem, stream, tmA, tmB, tmD, tmR, Q));
+  T2H_CUDA(launch_pdl(tapgemm_swap_kernel<kPair>, dim3(grid), dim3(kSwapThreads), kDynSmem, stream, tmA, tmB, tmD,
+                      tmR, Q));
   return T2H_OK;
 }
 
@@ -955,6 +960,17 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
   long long total = (long long)p->n_img * P.tiles_w * P.tiles_h * P.n_tiles_n;
   T2H_CHECK_ARG(total < (1LL << 31), "tapgemm: too many tiles");
   P.total_tiles = (int)total;
+  // Paired mode of the swapped kernel: one CTA computes two vertically adjacent tiles that share every weight tile
+  // and one slab, halving the weight bytes per output pixel.  It halves the number of work items too, so it is taken
+  // only when there are still at least as many pairs as SMs.  P.tiles_h then counts pairs of tile rows.
+  const bool pair = swap && P.total_tiles >= 2 * num_sms();
+  if (pair) {
+    P.slab_rows += TH;
+    T2H_CHECK_ARG(P.slab_rows * TW * 128 <= kSwapPairASlot, "tapgemm: paired slab of %d rows does not fit",
+                  P.slab_rows);
+    P.tiles_h = ceil_div(P.tiles_h, 2);
+    P.total_tiles = p->n_img * P.tiles_w * P.tiles_h * P.n_tiles_n;
+  }
 
   // ---- epilogue mode
   const int esz = (p->d_mode == T2H_OUT_F32) ? 4 : 2;
@@ -1079,7 +1095,7 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
   }
 
   cudaStream_t s = as_stream(stream);
-  if (swap) return launch_swap(tmA, tmB, tmD, tmR, P, s);
+  if (swap) return pair ? launch_swap<true>(tmA, tmB, tmD, tmR, P, s) : launch_swap<false>(tmA, tmB, tmD, tmR, P, s);
   switch (BN) {
     case 16: return launch<16>(tmA, tmB, tmD, tmR, P, s);
     case 32: return launch<32>(tmA, tmB, tmD, tmR, P, s);

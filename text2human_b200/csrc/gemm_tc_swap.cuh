@@ -10,12 +10,22 @@
 // is issued; the ring slots a group read last are released once the following group has been issued and the
 // group itself has completed (wgmma.wait_group 1).
 //
-// Epilogue, straight from the accumulator registers: thread t of warpgroup wg holds output channels
-// 64 wg + 16 (t / 32) + (t % 32) / 4 and that + 8, at pixels 8 j + 2 (t % 4) + {0, 1} of every 8-pixel block j, so
-// each consumer warp owns 16 channels x 128 pixels and finishes them alone (no block or warpgroup barrier):
-// +bias (two registers) -> activation -> +residual (its own TMA-loaded boxes) -> GroupNorm / norm-backward partial
-// sums (per thread, reduced over the four lanes of a channel and the channels of a group) -> st.shared into its own
-// 64-byte-swizzled [32 pixels][16 channels] boxes -> TMA store.
+// Paired mode (kPair): a work item is two vertically adjacent tiles (rows h0 and h0 + TH, same image and 128-channel
+// block).  Warpgroup wg computes tile wg for all 128 output channels: two M=64 wgmmas per K step, one per 64-channel
+// half of the weight tile, into two 64-register accumulators.  Both warpgroups read every weight tile, so each one
+// feeds 256 output pixels and the weight bytes per pixel halve; one slab of 2 TH + extra rows serves both tiles
+// (warpgroup 1's view starts TH TW 128 = 16 KB further in, a multiple of the 1024-byte swizzle period).  Per pixel the
+// MMA sequence is the unpaired one, so outputs are bit-identical; only the order of the fp64 sum atomics differs.
+// The second tile of a pair may lie partly or wholly below the image: TMA zero-fills its slab rows and residual boxes,
+// clips its stores, and pix_ok keeps it out of the sums.
+//
+// Epilogue, straight from the accumulator registers: thread t of a warpgroup holds, per 64-channel half it computes,
+// channels 16 (t / 32) + (t % 32) / 4 and that + 8 of the half, at pixels 8 j + 2 (t % 4) + {0, 1} of every 8-pixel
+// block j, so each consumer warp owns 16 channels x 128 pixels per half and finishes them alone (no block or
+// warpgroup barrier): +bias (two registers) -> activation -> +residual (its own TMA-loaded boxes) -> GroupNorm /
+// norm-backward partial sums (per thread, reduced over the four lanes of a channel and the channels of a group) ->
+// st.shared into its own 64-byte-swizzled [32 pixels][16 channels] boxes -> TMA store.  In paired mode a warp runs
+// this twice through the same boxes, once per half.
 #pragma once
 
 namespace t2h {
@@ -25,8 +35,11 @@ constexpr int kSwapBox = 32 * 16 * 4;         // one TMA box of the epilogue: 32
 constexpr int kSwapWarpBuf = 4 * kSwapBox;    // a consumer warp's 128 pixels: residual in, output out, in place
 static_assert(8 * kSwapWarpBuf == kEpiBytes, "epilogue boxes");
 constexpr int kSwapRingBytes = kDynSmem - 1024 - kEpiBytes;  // A ring + B ring
+// a paired-mode slab: 2 TH + 2 rows of TW positions (TH TW = 128, TW <= 16) x 128 bytes
+constexpr int kSwapPairASlot = (2 * 128 + 2 * 16) * 128;
+static_assert(kSwapPairASlot % 1024 == 0, "slab slots keep the 128-byte swizzle phase");
 // Register split (setmaxnreg): the producer warpgroup only issues TMA and waits on barriers; the consumers hold a
-// 64-register accumulator plus the epilogue's values.  The split redistributes what the CTA was launched with, 384
+// 64-register (paired: 128-register) accumulator plus the epilogue's values.  The split redistributes what the CTA was launched with, 384
 // threads x 168 registers (the __launch_bounds__ ceiling): 128 x 40 + 256 x 232.
 constexpr int kSwapProducerRegs = 40;
 constexpr int kSwapConsumerRegs = 232;
@@ -65,24 +78,42 @@ __device__ __forceinline__ void nb_flush(const TapGemmDev& P, int img, int c, in
   }
 }
 
-// Ring invariant: no group waits on a slot whose release is deferred behind it.  When a group's operands are waited
-// for, every slot whose last reader is two or more groups back has been released.  Each group reads one B tile and
-// the B index advances by at most one per group, so the tile a group needs reuses a slot released two groups back
-// whenever b_slots >= 2.  A slabs (3-product order hi.lo, hi.hi, lo.hi per tap): the next chunk's hi slab reuses the
-// slot of the current chunk's hi slab (last read by the hi.hi group before the chunk's final group) when
-// a_slots >= 2.  1-product: one slab per chunk, a_slots >= 2.
+// work item -> its (first) tile; in paired mode tiles_h counts pairs of tile rows
+template <bool kPair>
+__device__ __forceinline__ TileCoord decode_item(const TapGemmDev& P, int item) {
+  TileCoord t = decode_tile(P, item, 128);
+  if (kPair) t.h0 *= 2;
+  return t;
+}
+
+// Ring invariant (both modes; tests/test_swap_ring_model.py replays it).  Within one warpgroup, no group waits on a
+// slot whose release is deferred behind it: when a group's operands are waited for, every slot whose last reader is
+// two or more groups back has been released.  Each group reads one B tile and the B index advances by at most one
+// per group, so the tile a group needs reuses a slot released two groups back whenever b_slots >= 2.  A slabs
+// (3-product order hi.lo, hi.hi, lo.hi per tap): the next chunk's hi slab reuses the slot of the current chunk's hi
+// slab (last read by the hi.hi group before the chunk's final group) when a_slots >= 2.  1-product: one slab per
+// chunk, a_slots >= 2.
+// Across the two warpgroups: both read every slot (unpaired: one 64-row half of each weight tile, the same slab view;
+// paired: both halves of each weight tile, their own slab view), every slot's empty barrier counts all 256 consumer
+// threads, and both warpgroups wait on the fills in the same order.  So the warpgroup that is further behind never
+// waits on the other: every fill it waits for reuses a slot it has released itself (the invariant above) and the
+// other warpgroup, having passed that point, has released too.  The lag between the two is bounded by the ring
+// depth, and the leader simply waits for the fills the laggard's releases allow.
+template <bool kPair>
 __global__ void __launch_bounds__(kSwapThreads, 1)
 tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
                     const __grid_constant__ TapGemmDev P) {
   using C = Cfg<128>;
+  constexpr int kASlot = kPair ? kSwapPairASlot : C::kASlot;
+  constexpr int NH = kPair ? 2 : 1;  // 64-channel halves of the tile a consumer warpgroup computes
   pdl_launch_dependents();  // the next kernel may start its prologue once every CTA of this one is running
   const int NA = P.a_slots, NB = P.b_slots;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem =
       reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_ring = smem;
-  uint8_t* b_ring = smem + NA * C::kASlot;
+  uint8_t* b_ring = smem + NA * kASlot;
   uint8_t* epi_buf = b_ring + NB * C::kBSlot;  // 8 consumer warps x kSwapWarpBuf
 
   __shared__ __align__(8) uint64_t a_full[kMaxSlots];
@@ -116,9 +147,10 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   // everything above touched only shared memory and kernel parameters; from here on the previous
   // kernel's results are read (and buffers it may still be reading are overwritten)
   pdl_wait();
-  // tile schedule: round-robin over the CTAs, or -- when the epilogue accumulates per-image sums (nb_sums) -- one
-  // contiguous range per CTA, so that a CTA stays inside one image and flushes its sums once or twice per launch
-  // instead of once per tile (round-robin put ~1000 double atomics per launch on every (image, channel) address)
+  // work schedule (items: tiles, or pairs of tiles): round-robin over the CTAs, or -- when the epilogue accumulates
+  // per-image sums (nb_sums) -- one contiguous range per CTA, so that a CTA stays inside one image and flushes its sums
+  // once or twice per launch instead of once per item (round-robin put ~1000 double atomics per launch on every
+  // (image, channel) address)
   const bool contig = P.nb_sums != nullptr;
   const int tile_first = contig ? (int)((long long)blockIdx.x * P.total_tiles / gridDim.x) : (int)blockIdx.x;
   const int tile_end = contig ? (int)((long long)(blockIdx.x + 1) * P.total_tiles / gridDim.x) : P.total_tiles;
@@ -136,13 +168,13 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       if (lane == 0) {
         int sa = 0, pa = 0;
         for (int tile = tile_first; tile < tile_end; tile += tile_step) {
-          const TileCoord t = decode_tile(P, tile, 128);
+          const TileCoord t = decode_item<kPair>(P, tile);
           for (int g = 0; g < P.ngroups; ++g)
             for (int ch = 0; ch < P.kchunks; ++ch)
               for (int pl = 0; pl < a_planes; ++pl) {
                 mbar_wait(&a_empty[sa], pa ^ 1);
                 mbar_expect_tx(&a_full[sa], slab_bytes);
-                tma_load_4d(&tmA, &a_full[sa], a_ring + sa * C::kASlot, ch * kBK, t.w0 + P.g_dx[g],
+                tma_load_4d(&tmA, &a_full[sa], a_ring + sa * kASlot, ch * kBK, t.w0 + P.g_dx[g],
                             t.h0 + P.g_dy0[g], t.img + P.g_ioff[g] + pl * P.a_term_imgs);
                 if (++sa == NA) {
                   sa = 0;
@@ -156,7 +188,7 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       if (lane == 0) {
         int sb = 0, pb = 0;
         for (int tile = tile_first; tile < tile_end; tile += tile_step) {
-          const TileCoord t = decode_tile(P, tile, 128);
+          const TileCoord t = decode_item<kPair>(P, tile);
           for (int g = 0; g < P.ngroups; ++g)
             for (int ch = 0; ch < P.kchunks; ++ch)
               for (int tp = 0; tp < P.g_ntaps[g]; ++tp)
@@ -176,11 +208,13 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   } else {
     // ---------------------------------------------- consumers: D^T[cout, pixel] += W * slab^T, then the epilogue
     setmaxnreg_inc<kSwapConsumerRegs>();
-    const int wg = (warp - 4) >> 2;  // output channels 64 wg .. 64 wg + 63 of the tile
+    // unpaired: output channels 64 wg .. 64 wg + 63 of the tile; paired: all 128 channels of the pair's tile wg
+    const int wg = (warp - 4) >> 2;
+    const int q = (warp - 4) & 3;  // warp of the warpgroup: channels 16 q .. 16 q + 15 of each 64-channel half
     const uint32_t row16 = (uint32_t)(P.TW * 128) >> 4;  // one slab image row, in 16-byte units
-    const uint64_t x_desc0 = gmma_desc(smem_u32(a_ring));
-    const uint64_t w_desc0 = gmma_desc(smem_u32(b_ring) + 8192u * wg);
-    constexpr uint32_t A16 = C::kASlot >> 4, B16 = C::kBSlot >> 4;
+    const uint64_t x_desc0 = gmma_desc(smem_u32(a_ring) + (kPair ? 128u * 128u * wg : 0u));
+    const uint64_t w_desc0 = gmma_desc(smem_u32(b_ring) + (kPair ? 0u : 8192u * wg));
+    constexpr uint32_t A16 = kASlot >> 4, B16 = C::kBSlot >> 4, H16 = 8192u >> 4;
     const int ngroups = P.ngroups, kchunks = P.kchunks;
     int sa = 0, pa = 0, sb = 0, pb = 0;
     const int e = warp - 4;  // 0..7
@@ -193,33 +227,48 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     uint32_t res_par = 0;
     const int cpg = P.gn_cpg;
     const int red = 4 * (cpg < 8 ? cpg : 8);  // lanes holding one GroupNorm group's (channel, pixel) partial sums
+    // first of the 16 channels this warp finishes in half h of the column block at n0
+    auto chan0 = [&](int n0, int h) { return n0 + 64 * (kPair ? h : wg) + 16 * q; };
     // norm-backward sums: the "residual" tile is x and is not added
     const bool nb = P.nb_sums != nullptr;
-    // per thread: channel c (index 0) and c + 8 (index 1); the sums run on across consecutive tiles of the same
-    // (image, channel block) and are flushed when that changes
-    float nb_mean[2] = {0.f, 0.f}, nb_rstd[2] = {0.f, 0.f}, nb_ga[2] = {0.f, 0.f}, nb_be[2] = {0.f, 0.f};
-    float nb_s1[2] = {0.f, 0.f}, nb_s2[2] = {0.f, 0.f};
-    int nb_img = -1, nb_c = -1;
+    // per thread and half: channel c (index 0) and c + 8 (index 1); the sums run on across consecutive items of the
+    // same (image, channel block) and are flushed when that changes.  Their GroupNorm constants are derived again
+    // for every item: held across items, they would cost the paired accumulator 16 registers.
+    float nb_s1[NH][2], nb_s2[NH][2];
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+      for (int k = 0; k < 2; ++k) nb_s1[h][k] = nb_s2[h][k] = 0.f;
+    int nb_img = -1, nb_n0 = -1;
+    // residual (or x) boxes of half h of this warp's tile, into the boxes the previous stores read from
+    auto load_res = [&](const TileCoord& t, int h) {
+      tma_store_wait_read<0>();
+      mbar_expect_tx(&res_bar[e], kSwapWarpBuf);
+      for (int k = 0; k < 4; ++k)
+        tma_load_4d(&tmR, &res_bar[e], my_buf + k * kSwapBox, chan0(t.n0, h), t.w0, t.h0 + k * rows_per_box, t.img);
+    };
 
     for (int tile = tile_first; tile < tile_end; tile += tile_step) {
-      const TileCoord t = decode_tile(P, tile, 128);
-      const int c0 = t.n0 + 16 * e;       // this warp's 16 output channels
-      const int ca = c0 + (lane >> 2);    // this thread's channels: ca and ca + 8
+      TileCoord t = decode_item<kPair>(P, tile);
+      if (kPair) t.h0 += wg * P.TH;  // this warpgroup's tile of the pair
       if (has_res && lane == 0) {
-        // the tile's residual (or x) boxes load while its MMAs run, into the boxes the previous tile's output
-        // stores read from
-        tma_store_wait_read<0>();
-        mbar_expect_tx(&res_bar[e], kSwapWarpBuf);
-        for (int k = 0; k < 4; ++k)
-          tma_load_4d(&tmR, &res_bar[e], my_buf + k * kSwapBox, c0, t.w0, t.h0 + k * rows_per_box, t.img);
-        if (nb && tile + tile_step < tile_end) {
-          // the NEXT tile's x boxes go to L2 now, so that its loads above are L2 hits
-          const TileCoord tn = decode_tile(P, tile + tile_step, 128);
+        // half 0's boxes load while the MMAs run; later halves' go to L2 now, so that their loads are L2 hits
+        load_res(t, 0);
+#pragma unroll
+        for (int h = 1; h < NH; ++h)
           for (int k = 0; k < 4; ++k)
-            tma_prefetch_4d(&tmR, tn.n0 + 16 * e, tn.w0, tn.h0 + k * rows_per_box, tn.img);
+            tma_prefetch_4d(&tmR, chan0(t.n0, h), t.w0, t.h0 + k * rows_per_box, t.img);
+        if (nb && tile + tile_step < tile_end) {
+          // the NEXT item's x boxes go to L2 now, so that its loads above are L2 hits
+          TileCoord tn = decode_item<kPair>(P, tile + tile_step);
+          if (kPair) tn.h0 += wg * P.TH;
+#pragma unroll
+          for (int h = 0; h < NH; ++h)
+            for (int k = 0; k < 4; ++k)
+              tma_prefetch_4d(&tmR, chan0(tn.n0, h), tn.w0, tn.h0 + k * rows_per_box, tn.img);
         }
       }
-      float acc[64];
+      float acc[NH][64];
       {
         uint32_t accf = 0;
         int rel_b = -1, rel_a = -1;  // the slots the group in flight is the last reader of (-1: none)
@@ -227,7 +276,12 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         // then serialises every MMA); the arrivals are for the previous group, which wait_group 1 has completed
         auto group = [&](uint64_t w, uint64_t x, int last_b, int last_a) {
           wgmma_fence();
-          wgmma_chunk<0, 0>(acc, w, x, accf);
+#pragma unroll
+          for (int h = 0; h < NH; ++h) {
+            uint32_t f = accf;
+            wgmma_chunk<0, 0>(acc[h], w + h * H16, x, f);
+          }
+          accf = 1;
           wgmma_commit();
           wgmma_wait<1>();
           if (rel_b >= 0) mbar_arrive(&b_empty[rel_b]);
@@ -271,160 +325,185 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           }
         }
         wgmma_wait<0>();
-        wgmma_fence_regs(acc);
+#pragma unroll
+        for (int h = 0; h < NH; ++h) wgmma_fence_regs(acc[h]);
         if (rel_b >= 0) mbar_arrive(&b_empty[rel_b]);
         if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
       }
-      // accumulator element i: channel ca + 8 ((i >> 1) & 1), pixel 8 (i >> 2) + m2 + (i & 1); in-box pixel and
-      // channel of the [32][16] box i >> 4
-      auto box_off = [&](int i) { return (i >> 4) * kSwapBox + swz64(8 * ((i >> 2) & 3) + m2 + (i & 1), (lane >> 2) + 8 * ((i >> 1) & 1)); };
-      auto pix_ok = [&](int i) {
-        const int p = 8 * (i >> 2) + m2 + (i & 1);
-        return (t.h0 + (p >> tw_shift) < P.H) && (t.w0 + (p & (P.TW - 1)) < P.W);
-      };
       // interior tiles need no per-pixel validity test for the GroupNorm / norm-backward sums
       const bool interior = (t.h0 + P.TH <= P.H) && (t.w0 + P.TW <= P.W);
-      {
-        float bias2[2] = {0.f, 0.f};
-        if (P.bias_mode == T2H_BIAS_COL) {
-          if (ca < P.n_out) bias2[0] = __ldg(P.bias + t.img * P.bias_sn + ca);
-          if (ca + 8 < P.n_out) bias2[1] = __ldg(P.bias + t.img * P.bias_sn + ca + 8);
+      // bit 2 j + b: this thread's pixel 8 j + m2 + b lies inside the image (one register for both halves)
+      uint32_t ok_mask = ~0u;
+      if (!interior) {
+        ok_mask = 0;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const int p = 8 * (j >> 1) + m2 + (j & 1);
+          if ((t.h0 + (p >> tw_shift) < P.H) && (t.w0 + (p & (P.TW - 1)) < P.W)) ok_mask |= 1u << j;
         }
-#pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = acc[i] * P.alpha + bias2[(i >> 1) & 1];
       }
-      if (P.act == T2H_ACT_GELU) {
+      auto pix_ok = [&](int i) { return ((ok_mask >> (2 * (i >> 2) + (i & 1))) & 1u) != 0; };
+      if (nb && (t.img != nb_img || t.n0 != nb_n0)) {  // the previous (image, channel block)'s sums are flushed
 #pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = gelu_erf(acc[i]);
-      } else if (P.act == T2H_ACT_RELU) {
+        for (int h = 0; h < NH; ++h) {
+          if (nb_img >= 0)
+            nb_flush(P, nb_img, chan0(nb_n0, h) + (lane >> 2), lane, nb_s1[h][0], nb_s1[h][1], nb_s2[h][0],
+                     nb_s2[h][1]);
 #pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = fmaxf(acc[i], 0.f);
-      } else if (P.act == T2H_ACT_LRELU) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = acc[i] > 0.f ? acc[i] : 0.2f * acc[i];
+          for (int k = 0; k < 2; ++k) nb_s1[h][k] = nb_s2[h][k] = 0.f;
+        }
+        nb_img = t.img;
+        nb_n0 = t.n0;
       }
-      if (has_res) {
-        mbar_wait(&res_bar[e], res_par);
-        res_par ^= 1;
-        if (nb) {
-          // norm-backward constants of this thread's two channels in image t.img (mean, rstd from the forward
-          // statistics); the previous (image, channel block)'s sums are flushed first
-          if (t.img != nb_img || c0 != nb_c) {
-            if (nb_img >= 0) nb_flush(P, nb_img, nb_c + (lane >> 2), lane, nb_s1[0], nb_s1[1], nb_s2[0], nb_s2[1]);
-            nb_img = t.img;
-            nb_c = c0;
+#pragma unroll
+      for (int h = 0; h < NH; ++h) {
+        float(&a)[64] = acc[h];
+        const int c0 = chan0(t.n0, h);     // this warp's 16 output channels of the half
+        const int ca = c0 + (lane >> 2);  // this thread's channels: ca and ca + 8
+        if (h > 0 && has_res && lane == 0) load_res(t, h);
+        // accumulator element i: channel ca + 8 ((i >> 1) & 1), pixel 8 (i >> 2) + m2 + (i & 1); in-box pixel and
+        // channel of the [32][16] box i >> 4
+        auto box_off = [&](int i) { return (i >> 4) * kSwapBox + swz64(8 * ((i >> 2) & 3) + m2 + (i & 1), (lane >> 2) + 8 * ((i >> 1) & 1)); };
+        {
+          float bias2[2] = {0.f, 0.f};
+          if (P.bias_mode == T2H_BIAS_COL) {
+            if (ca < P.n_out) bias2[0] = __ldg(P.bias + t.img * P.bias_sn + ca);
+            if (ca + 8 < P.n_out) bias2[1] = __ldg(P.bias + t.img * P.bias_sn + ca + 8);
+          }
+#pragma unroll
+          for (int i = 0; i < 64; ++i) a[i] = a[i] * P.alpha + bias2[(i >> 1) & 1];
+        }
+        if (P.act == T2H_ACT_GELU) {
+#pragma unroll
+          for (int i = 0; i < 64; ++i) a[i] = gelu_erf(a[i]);
+        } else if (P.act == T2H_ACT_RELU) {
+#pragma unroll
+          for (int i = 0; i < 64; ++i) a[i] = fmaxf(a[i], 0.f);
+        } else if (P.act == T2H_ACT_LRELU) {
+#pragma unroll
+          for (int i = 0; i < 64; ++i) a[i] = a[i] > 0.f ? a[i] : 0.2f * a[i];
+        }
+        if (has_res) {
+          mbar_wait(&res_bar[e], res_par);
+          res_par ^= 1;
+          if (nb) {
+            // norm-backward constants of this thread's two channels in image t.img (mean, rstd from the forward
+            // statistics)
+            float nb_mean[2], nb_rstd[2], nb_ga[2], nb_be[2];
             const int ncpg = P.n_out / P.nb_groups;
             const double cnt = (double)P.H * P.W * ncpg;
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              nb_s1[h] = 0.f;
-              nb_s2[h] = 0.f;
-              const int c = min(ca + 8 * h, P.n_out - 1);
+            for (int k = 0; k < 2; ++k) {
+              const int c = min(ca + 8 * k, P.n_out - 1);
               const double* st = P.nb_stats + ((long long)t.img * P.nb_groups + c / ncpg) * 2;
               const double m = st[0] / cnt;
               double var = st[1] / cnt - m * m;
               if (var < 0) var = 0;
-              nb_mean[h] = (float)m;
-              nb_rstd[h] = (float)(1.0 / sqrt(var + (double)P.nb_eps));
-              nb_ga[h] = __ldg(P.nb_gamma + c);
-              nb_be[h] = __ldg(P.nb_beta + c);
+              nb_mean[k] = (float)m;
+              nb_rstd[k] = (float)(1.0 / sqrt(var + (double)P.nb_eps));
+              nb_ga[k] = __ldg(P.nb_gamma + c);
+              nb_be[k] = __ldg(P.nb_beta + c);
             }
-          }
-          // acc = dL/d act(norm(x)); accumulate pass 1 of the norm backward: sum du, sum du*xhat over the pixels.
-          // Pixels outside the image are zeroed up front (their x boxes are zero-filled), the activation is chosen
-          // outside the element loop.
-          if (!interior) {
+            // acc = dL/d act(norm(x)); accumulate pass 1 of the norm backward: sum du, sum du*xhat over the pixels.
+            // Pixels outside the image are zeroed up front (their x boxes are zero-filled), the activation is chosen
+            // outside the element loop.
+            if (!interior) {
 #pragma unroll
-            for (int i = 0; i < 64; ++i)
-              if (!pix_ok(i)) acc[i] = 0.f;
-          }
-          if (P.nb_act == 1) {
+              for (int i = 0; i < 64; ++i)
+                if (!pix_ok(i)) a[i] = 0.f;
+            }
+            if (P.nb_act == 1) {
 #pragma unroll
-            for (int i = 0; i < 64; ++i) {
-              const int h = (i >> 1) & 1;
-              const float xh = (lds_f32(buf_s + box_off(i)) - nb_mean[h]) * nb_rstd[h];
-              const float du = acc[i] * act_grad_fast(fmaf(xh, nb_ga[h], nb_be[h]), 1);
-              nb_s1[h] += du;
-              nb_s2[h] = fmaf(du, xh, nb_s2[h]);
+              for (int i = 0; i < 64; ++i) {
+                const int k = (i >> 1) & 1;
+                const float xh = (lds_f32(buf_s + box_off(i)) - nb_mean[k]) * nb_rstd[k];
+                const float du = a[i] * act_grad_fast(fmaf(xh, nb_ga[k], nb_be[k]), 1);
+                nb_s1[h][k] += du;
+                nb_s2[h][k] = fmaf(du, xh, nb_s2[h][k]);
+              }
+            } else {
+              const int an = P.nb_act;
+#pragma unroll
+              for (int i = 0; i < 64; ++i) {
+                const int k = (i >> 1) & 1;
+                const float xh = (lds_f32(buf_s + box_off(i)) - nb_mean[k]) * nb_rstd[k];
+                const float du = a[i] * ((an == 2 && fmaf(xh, nb_ga[k], nb_be[k]) <= 0.f) ? 0.2f : 1.0f);
+                nb_s1[h][k] += du;
+                nb_s2[h][k] = fmaf(du, xh, nb_s2[h][k]);
+              }
             }
           } else {
-            const int a = P.nb_act;
 #pragma unroll
-            for (int i = 0; i < 64; ++i) {
-              const int h = (i >> 1) & 1;
-              const float xh = (lds_f32(buf_s + box_off(i)) - nb_mean[h]) * nb_rstd[h];
-              const float du = acc[i] * ((a == 2 && fmaf(xh, nb_ga[h], nb_be[h]) <= 0.f) ? 0.2f : 1.0f);
-              nb_s1[h] += du;
-              nb_s2[h] = fmaf(du, xh, nb_s2[h]);
+            for (int i = 0; i < 64; ++i) a[i] += lds_f32(buf_s + box_off(i));
+          }
+        }
+        if (P.gn_stats) {
+          float gs[2] = {0.f, 0.f}, gss[2] = {0.f, 0.f};
+#pragma unroll
+          for (int i = 0; i < 64; ++i) {
+            const float x = (interior || pix_ok(i)) ? a[i] : 0.f;
+            gs[(i >> 1) & 1] += x;
+            gss[(i >> 1) & 1] = fmaf(x, x, gss[(i >> 1) & 1]);
+          }
+          // lanes 4c .. 4c + 3 hold channel c's pixels; the channels of a group are consecutive lane quads
+          for (int off = 1; off < red; off <<= 1) {
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+              gs[k] += __shfl_xor_sync(0xffffffffu, gs[k], off);
+              gss[k] += __shfl_xor_sync(0xffffffffu, gss[k], off);
             }
           }
-        } else {
+          if (cpg >= 16) {  // channels ca and ca + 8 are in the same group
+            gs[0] += gs[1];
+            gss[0] += gss[1];
+          }
+          if ((lane & (red - 1)) == 0) {
 #pragma unroll
-          for (int i = 0; i < 64; ++i) acc[i] += lds_f32(buf_s + box_off(i));
-        }
-      }
-      if (P.gn_stats) {
-        float gs[2] = {0.f, 0.f}, gss[2] = {0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < 64; ++i) {
-          const float x = (interior || pix_ok(i)) ? acc[i] : 0.f;
-          gs[(i >> 1) & 1] += x;
-          gss[(i >> 1) & 1] = fmaf(x, x, gss[(i >> 1) & 1]);
-        }
-        // lanes 4c .. 4c + 3 hold channel c's pixels; the channels of a group are consecutive lane quads
-        for (int off = 1; off < red; off <<= 1) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            gs[h] += __shfl_xor_sync(0xffffffffu, gs[h], off);
-            gss[h] += __shfl_xor_sync(0xffffffffu, gss[h], off);
+            for (int k = 0; k < 2; ++k) {
+              if (k == 1 && cpg >= 16) break;
+              double* dst = P.gn_stats + ((long long)t.img * P.gn_groups + (ca + 8 * k) / cpg) * 2;
+              atomicAdd(dst, (double)gs[k]);
+              atomicAdd(dst + 1, (double)gss[k]);
+            }
           }
         }
-        if (cpg >= 16) {  // channels ca and ca + 8 are in the same group
-          gs[0] += gs[1];
-          gss[0] += gss[1];
-        }
-        if ((lane & (red - 1)) == 0) {
+        if (P.epi_mode == EPI_DIRECT) {
+          // strided destination (NCHW conv_out, Cout < 128): the threads of valid channels store their pixels
+          float* dst = reinterpret_cast<float*>(P.d) + (long long)t.img * P.d_sn;
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (h == 1 && cpg >= 16) break;
-            double* dst = P.gn_stats + ((long long)t.img * P.gn_groups + (ca + 8 * h) / cpg) * 2;
-            atomicAdd(dst, (double)gs[h]);
-            atomicAdd(dst + 1, (double)gss[h]);
+          for (int i = 0; i < 64; ++i) {
+            const int c = ca + 8 * ((i >> 1) & 1);
+            const int p = 8 * (i >> 2) + m2 + (i & 1);
+            const int hh = t.h0 + (p >> tw_shift), w = t.w0 + (p & (P.TW - 1));
+            if (c < P.n_out && hh < P.H && w < P.W) dst[(long long)c * P.d_sc + (long long)hh * P.d_sh + (long long)w * P.d_sw] = a[i];
           }
+          continue;
         }
-      }
-      if (P.epi_mode == EPI_DIRECT) {
-        // strided destination (NCHW conv_out, Cout < 128): the threads of valid channels store their pixels
-        float* dst = reinterpret_cast<float*>(P.d) + (long long)t.img * P.d_sn;
+        // Output boxes, written in place of the residual boxes they were added from.  Per st.shared the 32 lanes
+        // write 8 channels x 4 pixels of one pixel parity; the 64-byte swizzle puts them on 16 banks, 2 lanes each:
+        // 2-way bank conflicts.
 #pragma unroll
-        for (int i = 0; i < 64; ++i) {
-          const int c = ca + 8 * ((i >> 1) & 1);
-          const int p = 8 * (i >> 2) + m2 + (i & 1);
-          const int h = t.h0 + (p >> tw_shift), w = t.w0 + (p & (P.TW - 1));
-          if (c < P.n_out && h < P.H && w < P.W) dst[(long long)c * P.d_sc + (long long)h * P.d_sh + (long long)w * P.d_sw] = acc[i];
-        }
-        continue;
-      }
-      // Output boxes, written in place of the residual boxes they were added from.  Per st.shared the 32 lanes
-      // write 8 channels x 4 pixels of one pixel parity; the 64-byte swizzle puts them on 16 banks, 2 lanes each:
-      // 2-way bank conflicts.
+        for (int k = 0; k < 4; ++k) {
+          if (!has_res) {
+            if (lane == 0) tma_store_wait_read<3>();  // the store that last read this box (4 commits ago) is done
+            __syncwarp();
+          }
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if (!has_res) {
-          if (lane == 0) tma_store_wait_read<3>();  // the store that last read this box (4 commits ago) is done
+          for (int i = 16 * k; i < 16 * k + 16; ++i) sts_f32(buf_s + box_off(i), a[i]);
+          fence_proxy_async_smem();
           __syncwarp();
-        }
-#pragma unroll
-        for (int i = 16 * k; i < 16 * k + 16; ++i) sts_f32(buf_s + box_off(i), acc[i]);
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_4d(&tmD, my_buf + k * kSwapBox, c0, t.w0, t.h0 + k * rows_per_box, t.img);
-          tma_store_commit();
+          if (lane == 0) {
+            tma_store_4d(&tmD, my_buf + k * kSwapBox, c0, t.w0, t.h0 + k * rows_per_box, t.img);
+            tma_store_commit();
+          }
         }
       }
     }
-    if (nb && nb_img >= 0) nb_flush(P, nb_img, nb_c + (lane >> 2), lane, nb_s1[0], nb_s1[1], nb_s2[0], nb_s2[1]);
+    if (nb && nb_img >= 0) {
+#pragma unroll
+      for (int h = 0; h < NH; ++h)
+        nb_flush(P, nb_img, chan0(nb_n0, h) + (lane >> 2), lane, nb_s1[h][0], nb_s1[h][1], nb_s2[h][0], nb_s2[h][1]);
+    }
     if (lane == 0) tma_store_wait_read<0>();
   }
 }
