@@ -268,7 +268,7 @@ extern "C" int t2h_attn_fwd(const void* qkv, int terms, int64_t plane, int64_t l
   memset(&P, 0, sizeof(P));
   P.tokens = tokens;
   P.heads = heads;
-  P.qblocks = tokens / 128;
+  P.qblocks = tokens / 128;  // (tests/test_gpu_row_kernels.py::attn_route restates the grid)
   P.nchunks = tokens / 64;
   P.terms = terms;
   P.q_col = q_col;

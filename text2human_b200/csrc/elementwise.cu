@@ -794,6 +794,7 @@ int t2h_softmax_rows(const float* s, void* out, int64_t rows, int cols, float sc
   __half* o = reinterpret_cast<__half*>(out);
   const long long plane = rows * cols;
   cudaStream_t st = as_stream(stream);
+  // (tests/test_gpu_row_kernels.py::softmax_rows_route restates this choice)
   if (cols <= 512)
     T2H_CUDA(launch_pdl(softmax_rows_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, s, o, rows, cols, scale, terms, plane));
   else
@@ -812,6 +813,7 @@ int t2h_layernorm(const float* x, const float* gamma, const float* beta, void* o
   __half* o = reinterpret_cast<__half*>(out);
   const long long plane = rows * c;
   cudaStream_t st = as_stream(stream);
+  // (tests/test_gpu_row_kernels.py::layernorm_route restates this choice)
   if (c <= 512)
     T2H_CUDA(launch_pdl(layernorm_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, x, gamma, beta, o, rows, c, eps, terms, plane,
                         static_cast<const long long*>(nullptr)));
@@ -834,6 +836,7 @@ int t2h_splitk_reduce_ln(const float* partials, int n_slabs, int64_t slab, const
   const long long plane = (long long)ln_rows * c;
   const long long* rm = reinterpret_cast<const long long*>(row_map);
   cudaStream_t st = as_stream(stream);
+  // (tests/test_gpu_row_kernels.py::splitk_route restates the alignment rule and the choice of kernel below)
   const bool aligned = (c % 4 == 0) && (slab % 4 == 0) && ((reinterpret_cast<uintptr_t>(partials) | reinterpret_cast<uintptr_t>(x_out) |
                                                            reinterpret_cast<uintptr_t>(residual) | reinterpret_cast<uintptr_t>(bias) |
                                                            reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) % 16 == 0) &&
@@ -936,6 +939,7 @@ int t2h_layernorm_scatter(const float* x, const float* gamma, const float* beta,
   const long long plane = out_rows * c;
   const long long* rm = reinterpret_cast<const long long*>(row_map);
   cudaStream_t st = as_stream(stream);
+  // (tests/test_gpu_row_kernels.py::layernorm_route restates this choice)
   if (c <= 512)
     T2H_CUDA(launch_pdl(layernorm_kernel<16>, dim3(grid), dim3(warps * 32), 0, st, x, gamma, beta, o, rows, c, eps,
                         terms, plane, rm));

@@ -447,7 +447,7 @@ int t2h_planes_transpose(const void* x, void* out, int g, int r, int c, int64_t 
 
 int t2h_colsum(const float* x, float* out, int64_t rows, int c, t2h_stream_t stream) {
   T2H_CHECK_ARG(x && out && rows > 0 && c > 0, "colsum: bad args");
-  int rpb = 64;
+  int rpb = 64;  // (tests/test_gpu_row_kernels.py::colsum_route restates this grid)
   if (ceil_div64(rows, rpb) > 16384) rpb = (int)ceil_div64(rows, 16384);  // grid.y limit; conv bias gradients have millions of rows
   dim3 grid(ceil_div(c, 128), (unsigned)ceil_div64(rows, rpb));
   colsum_kernel<<<grid, 128, 0, as_stream(stream)>>>(x, out, rows, c, rpb);
@@ -493,6 +493,7 @@ static int layernorm_bwd_impl(const float* dy, const float* x, const float* gamm
                               float* dx_colsum, t2h_stream_t stream) {
   T2H_CHECK_ARG(dy && x && gamma && dx && dgamma && dbeta && rows > 0 && c > 0, "layernorm_bwd: bad args");
   T2H_CHECK_ARG(c <= 1024, "layernorm_bwd: C=%d > 1024 unsupported", c);
+  // (tests/test_gpu_row_kernels.py::layernorm_bwd_route restates the grid and the choice of kernel below)
   const int warps = 8;
   long long want = ceil_div64(rows, warps * 2);  // 2 rows per warp, 16 per block: enough warps in flight to
   const int grid = (int)(want < 1 ? 1 : want);   // cover HBM latency, 16x fewer global atomics than per-row
@@ -531,6 +532,7 @@ static int softmax_bwd_impl(const void* p, const float* dp, float* ds, void* ds_
   const int grid = (int)ceil_div64(rows, warps);
   cudaStream_t st = as_stream(stream);
   const __half* ph = reinterpret_cast<const __half*>(p);
+  // (tests/test_gpu_row_kernels.py::softmax_bwd_route restates this choice)
   if (cols <= 512)
     softmax_bwd_kernel<8><<<grid, warps * 32, 0, st>>>(ph, dp, ds, rows, cols, scale, terms, rows * cols,
                                                       reinterpret_cast<__half*>(ds_planes), out_scale);
