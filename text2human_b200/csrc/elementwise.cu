@@ -635,6 +635,7 @@ __global__ void u8_to_planes_kernel(const unsigned char* __restrict__ x, __half*
   }
 }
 
+// (tests/test_gpu_image_kernels.py::grid_route restates this rule)
 static inline int grid_for(long long work, int block) {
   long long g = ceil_div64(work, block);
   long long cap = (long long)num_sms() * 16;
@@ -644,7 +645,8 @@ static inline int grid_for(long long work, int block) {
 
 // Per-row argmax inside the row's own head (bot_index_prediction, sample_model.py:183-213):
 // logits [G][M][ncls]; row m reads head[m]'s slice and returns the lowest index of the maximum (-1 when
-// head[m] is outside 0..G-1).  One warp per row.
+// head[m] is outside 0..G-1).  NaN logits are skipped (torch.argmax would return the first NaN); a row with no
+// value above -inf gives 0 (tests/test_gpu_image_kernels.py::test_argmax_heads_rule pins this).  One warp per row.
 __global__ void argmax_heads_kernel(const float* __restrict__ logits, const long long* __restrict__ head,
                                     long long* __restrict__ out, long long M, int G, int ncls) {
   const long long m = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -726,7 +728,7 @@ int t2h_f32_to_planes(const float* x, void* out, int n, int h, int w, int c, int
   long long out_elems = (long long)n * h * w * c;
   if (mode == T2H_CVT_UP2X || mode == T2H_CVT_BILINEAR2X) out_elems *= 4;
   if (mode == T2H_CVT_MAXPOOL2) out_elems = (long long)n * (h / 2) * (w / 2) * c;
-  const long long work = out_elems / 8;
+  const long long work = out_elems / 8;  // (tests/test_gpu_image_kernels.py::f32_to_planes_route restates this grid)
   f32_to_planes_kernel<<<grid_for(work, 256), 256, 0, as_stream(stream)>>>(
       x, reinterpret_cast<__half*>(out), n, h, w, c, mode, terms, out_elems);
   T2H_LAUNCH_OK();
@@ -762,6 +764,7 @@ int t2h_gn_apply(const float* x, const double* stats, const float* gamma, const 
   T2H_CHECK_ARG(c % groups == 0 && c % 8 == 0 && c <= 4096, "gn_apply: C=%d groups=%d unsupported", c,
                 groups);
   T2H_CHECK_ARG(terms == 1 || terms == 2, "gn_apply: terms=%d", terms);
+  // (tests/test_gpu_image_kernels.py::gn_apply_route restates the blocks and pixels per block below)
   int blocks_x = ceil_div(num_sms() * 8, n);
   int ppb = ceil_div(hw, blocks_x);
   if (ppb < 16) ppb = 16;
@@ -778,7 +781,7 @@ int t2h_add_inplace(float* x, const float* y, int64_t numel, t2h_stream_t stream
   T2H_CHECK_ARG(x && y && numel > 0, "add_inplace: bad args");
   T2H_CHECK_ARG(reinterpret_cast<uintptr_t>(x) % 16 == 0 && reinterpret_cast<uintptr_t>(y) % 16 == 0,
                 "add_inplace: pointers must be 16-byte aligned");
-  const long long n4 = numel / 4;
+  const long long n4 = numel / 4;  // (tests/test_gpu_image_kernels.py::add_inplace_route restates the float4 loop and the tail)
   add_inplace_kernel<<<grid_for(n4 > 0 ? n4 : 1, 256), 256, 0, as_stream(stream)>>>(x, y, n4, numel);
   T2H_LAUNCH_OK();
   return T2H_OK;

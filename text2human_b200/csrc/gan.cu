@@ -13,6 +13,7 @@ struct alignas(16) H8 {
   __half v[8];
 };
 
+// (tests/test_gpu_image_kernels.py::grid_route restates this rule)
 static inline int grid_cap(long long work, int block, int per_sm = 16) {
   long long g = ceil_div64(work, block);
   long long cap = (long long)num_sms() * per_sm;
@@ -202,7 +203,9 @@ __global__ void bn_running_kernel(const double* __restrict__ stats, float* __res
   rvar[c] = (1.f - momentum) * rvar[c] + momentum * (float)unb;
 }
 
-// dpre = dy * (y > 0 ? 1 : slope) where y = LeakyReLU(pre) (sign preserved) given as the hi plane of its fp16 planes
+// dpre = dy * (y > 0 ? 1 : slope) where y = LeakyReLU(pre) (sign preserved) given as the hi plane of its fp16 planes.
+// The slope is read from hi: 0 < y <= 2^-25 rounds to an fp16 0 and gets 0.2 where autograd uses 1 (planes cannot
+// tell those y from 0; tests/test_gpu_image_kernels.py::test_lrelu_bwd_bit_exact pins this rule)
 __global__ void lrelu_bwd_kernel(const __half* __restrict__ y, const float* __restrict__ dy,
                                  float* __restrict__ dpre, __half* __restrict__ planes, int terms, long long n) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
@@ -691,6 +694,7 @@ int t2h_vq_bwd(const float* z, const float* codebook, const int64_t* idx, const 
 int t2h_l1_loss(const float* x, const float* xrec, float* grad, double* sum, int64_t n, float gscale,
                 t2h_stream_t stream) {
   T2H_CHECK_ARG(x && xrec && sum && n > 0, "l1_loss: bad args");
+  // (tests/test_gpu_image_kernels.py::loss_route restates this grid, as for hinge_kernel)
   l1_kernel<<<grid_cap(n, 256, 4), 256, 0, as_stream(stream)>>>(x, xrec, grad, sum, n, gscale);
   T2H_LAUNCH_OK();
   return T2H_OK;
@@ -704,7 +708,7 @@ int t2h_bce_logits(const float* logits, const float* ids, int n, int h, int w, i
   const long long npix = (long long)n * h * w;
   const int c8 = c_pad / 8;
   // whole warps (block_add) and a whole number of pixels per block (fixed channels per thread)
-  const int block = 32 * c8 * (c8 < 8 ? 8 / c8 : 1);
+  const int block = 32 * c8 * (c8 < 8 ? 8 / c8 : 1);  // (tests/test_gpu_image_kernels.py::bce_route restates this choice)
   bce_logits_kernel<<<grid_cap(npix, block / c8, 4), block, c_pad * sizeof(double), as_stream(stream)>>>(
       logits, ids, npix, c, c_pad, gscale, loss_sum, reinterpret_cast<__half*>(grad_planes), terms, colsum);
   T2H_LAUNCH_OK();
@@ -724,7 +728,7 @@ int t2h_diffaug_fwd(const float* x, const float* r, const int32_t* t, double* ss
   T2H_CHECK_ARG(x && r && t && ssum && out && b > 0 && h > 0 && w > 0, "diffaug_fwd: bad args");
   cudaStream_t st = as_stream(stream);
   T2H_CUDA(cudaMemsetAsync(ssum, 0, sizeof(double) * b, st));
-  const long long per = 3LL * h * w;
+  const long long per = 3LL * h * w;  // (tests/test_gpu_image_kernels.py::diffaug_route restates both capped grids)
   const int gx = grid_cap(per, 256, 2) < 64 ? grid_cap(per, 256, 2) : 64;
   sample_sum_kernel<<<dim3(gx, b), 256, 0, st>>>(x, ssum, per);
   T2H_LAUNCH_OK();
@@ -750,6 +754,7 @@ int t2h_diffaug_bwd(const float* dout, const float* r, const int32_t* t, double*
 int t2h_adaptive_weight(const float* rg, const float* gg, int64_t n, float inv_scale, float wmax, float enable,
                         float* out, t2h_stream_t stream) {
   T2H_CHECK_ARG(rg && gg && out && n > 0, "adaptive_weight: bad args");
+  // (tests/test_gpu_image_kernels.py::adaptive_weight_route restates this single block)
   adaptive_weight_kernel<<<1, 1024, 0, as_stream(stream)>>>(rg, gg, n, inv_scale, wmax, enable, out);
   T2H_LAUNCH_OK();
   return T2H_OK;

@@ -63,7 +63,7 @@ __global__ void vq_code_norms_kernel(const float* __restrict__ cb, float* __rest
   if (lane == 0) ee[code] = acc;
 }
 
-// Single-block counting sort of rows by codebook id + tile table.
+// Single-block counting sort of rows by codebook id + tile table (tests/test_gpu_image_kernels.py::vq_bin_route restates it).
 // ws layout (int32): [0]=n_tiles, [1..]=tile_book[maxT], tile_start[maxT], tile_cnt[maxT], perm[rows]
 __global__ void vq_bin_kernel(const int* __restrict__ book_id, int rows, int n_books, int maxT,
                               int* __restrict__ ws) {
