@@ -252,10 +252,9 @@ __global__ void gn_apply_kernel(const float* __restrict__ x, const double* __res
   const long long work = (long long)min((long long)pix_per_block, HW - p_begin) * c8;
   const float* xb = x + ((long long)n * HW + p_begin) * C;
   const long long ob = ((long long)n * HW + p_begin) * C;
-  for (long long i = threadIdx.x; i < work; i += blockDim.x) {
-    const int cc = (int)(i % c8);
-    float f[8];
-    load8(xb + i * 8, f);
+  // two 8-channel vectors per thread and iteration, both loaded before either is used: twice the bytes in flight
+  auto apply8 = [&](long long i, float (&f)[8]) {
+    const int cc = (int)((unsigned)i % (unsigned)c8);  // (work < 2^31: pix_per_block * C / 8)
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       float y = f[e] * scale[cc * 8 + e] + shift[cc * 8 + e];
@@ -264,6 +263,14 @@ __global__ void gn_apply_kernel(const float* __restrict__ x, const double* __res
       f[e] = y;
     }
     store_split8(f, out, ob + i * 8, plane, terms);
+  };
+  for (long long i = threadIdx.x; i < work; i += 2 * blockDim.x) {
+    const long long i2 = i + blockDim.x;
+    float f[8], g[8];
+    load8(xb + i * 8, f);
+    if (i2 < work) load8(xb + i2 * 8, g);
+    apply8(i, f);
+    if (i2 < work) apply8(i2, g);
   }
 }
 

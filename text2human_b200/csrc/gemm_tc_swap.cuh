@@ -11,22 +11,30 @@
 // group itself has completed (wgmma.wait_group 1).
 //
 // Paired mode (kPair): a work item is two vertically adjacent tiles (rows h0 and h0 + TH, same image and 128-channel
-// block).  Warpgroup wg computes tile wg for all 128 output channels: two M=64 wgmmas per K step, one per 64-channel
-// half of the weight tile, into two 64-register accumulators.  Both warpgroups read every weight tile, so each one
-// feeds 256 output pixels and the weight bytes per pixel halve; one slab of 2 TH + extra rows serves both tiles
-// (warpgroup 1's view starts TH TW 128 = 16 KB further in, a multiple of the 1024-byte swizzle period).  Per pixel the
-// MMA sequence is the unpaired one, so outputs are bit-identical; only the order of the fp64 sum atomics differs.
+// block).  One slab of 2 TH + extra rows serves both tiles: the second tile's view starts TH TW 128 = 16 KB after the
+// first's (a multiple of the 1024-byte swizzle period), so the two views are one 256-row K-major operand.  Warpgroup
+// wg computes channels 64 wg .. 64 wg + 63 of both tiles with one m64n256k16 wgmma per K step, into one 128-register
+// accumulator (registers 64 h .. 64 h + 63: tile h).  Each weight tile feeds 256 output pixels, so the weight bytes
+// per pixel halve, and a K step reads 2 KB of weights + 8 KB of slab from shared memory per 128 tensor-pipe clocks
+// (80 B/clk of the SM's 128; two m64n128k16 on 128-pixel views read 96).  Per output element the MMA sequence is the
+// unpaired one, so outputs are bit-identical; only the order of the fp64 sum atomics differs.
 // The second tile of a pair may lie partly or wholly below the image: TMA zero-fills its slab rows and residual boxes,
 // clips its stores, and pix_ok keeps it out of the sums.
 //
-// Epilogue, straight from the accumulator registers: thread t of a warpgroup holds, per 64-channel half it computes,
-// channels 16 (t / 32) + (t % 32) / 4 and that + 8 of the half, at pixels 8 j + 2 (t % 4) + {0, 1} of every 8-pixel
-// block j, so each consumer warp owns 16 channels x 128 pixels per half and finishes them alone (no block or
-// warpgroup barrier): +bias (two registers) -> activation -> +residual (its own TMA-loaded boxes) -> GroupNorm /
-// norm-backward partial sums (per thread, reduced over the four lanes of a channel and the channels of a group) ->
-// st.shared into its own 64-byte-swizzled [32 pixels][16 channels] boxes -> TMA store.  In paired mode a warp runs
-// this twice through the same boxes, once per half.
+// A warpgroup whose 64 channels all lie at or beyond n_out (warpgroup 1 of a column block with n0 + 64 >= n_out: the
+// 3-channel conv_out) has nothing to compute: it issues no wgmma and runs no epilogue for the item, and only keeps
+// the rings' barrier protocol (it waits on every fill and releases every slot, in the same order).
+//
+// Epilogue, straight from the accumulator registers: thread t of a warpgroup holds channels 16 (t / 32) + (t % 32) / 4
+// and that + 8 of the warpgroup's 64, at pixels 8 j + 2 (t % 4) + {0, 1} of every 8-pixel block j of each tile, so
+// each consumer warp owns 16 channels x 128 pixels per tile and finishes them alone (no block or warpgroup barrier):
+// +bias (two registers) -> activation -> +residual (its own TMA-loaded boxes) -> GroupNorm / norm-backward partial
+// sums (per thread, reduced over the four lanes of a channel and the channels of a group) -> st.shared into its own
+// 64-byte-swizzled [32 pixels][16 channels] boxes -> TMA store.  In paired mode a warp runs this twice through the
+// same boxes, once per tile, and reduces the GroupNorm sums of both tiles together.
 #pragma once
+
+#include <type_traits>
 
 namespace t2h {
 
@@ -93,9 +101,10 @@ __device__ __forceinline__ TileCoord decode_item(const TapGemmDev& P, int item) 
 // (3-product order hi.lo, hi.hi, lo.hi per tap): the next chunk's hi slab reuses the slot of the current chunk's hi
 // slab (last read by the hi.hi group before the chunk's final group) when a_slots >= 2.  1-product: one slab per
 // chunk, a_slots >= 2.
-// Across the two warpgroups: both read every slot (unpaired: one 64-row half of each weight tile, the same slab view;
-// paired: both halves of each weight tile, their own slab view), every slot's empty barrier counts all 256 consumer
-// threads, and both warpgroups wait on the fills in the same order.  So the warpgroup that is further behind never
+// Across the two warpgroups: both read every slot (one 64-row half of each weight tile and the same slab view, 128
+// rows unpaired and 256 paired; a paired group is still one group on the same slots, and a warpgroup with no valid
+// channel reads nothing but waits and releases alike), every slot's empty barrier counts all 256 consumer threads,
+// and both warpgroups wait on the fills in the same order.  So the warpgroup that is further behind never
 // waits on the other: every fill it waits for reuses a slot it has released itself (the invariant above) and the
 // other warpgroup, having passed that point, has released too.  The lag between the two is bounded by the ring
 // depth, and the leader simply waits for the fills the laggard's releases allow.
@@ -106,7 +115,7 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                     const __grid_constant__ TapGemmDev P) {
   using C = Cfg<128>;
   constexpr int kASlot = kPair ? kSwapPairASlot : C::kASlot;
-  constexpr int NH = kPair ? 2 : 1;  // 64-channel halves of the tile a consumer warpgroup computes
+  constexpr int NT = kPair ? 2 : 1;  // tiles of a work item: a consumer warpgroup computes 64 channels of each
   pdl_launch_dependents();  // the next kernel may start its prologue once every CTA of this one is running
   const int NA = P.a_slots, NB = P.b_slots;
   extern __shared__ uint8_t smem_raw[];
@@ -208,13 +217,12 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   } else {
     // ---------------------------------------------- consumers: D^T[cout, pixel] += W * slab^T, then the epilogue
     setmaxnreg_inc<kSwapConsumerRegs>();
-    // unpaired: output channels 64 wg .. 64 wg + 63 of the tile; paired: all 128 channels of the pair's tile wg
-    const int wg = (warp - 4) >> 2;
-    const int q = (warp - 4) & 3;  // warp of the warpgroup: channels 16 q .. 16 q + 15 of each 64-channel half
+    const int wg = (warp - 4) >> 2;  // output channels 64 wg .. 64 wg + 63 of the item's tile(s)
+    const int q = (warp - 4) & 3;    // warp of the warpgroup: channels 16 q .. 16 q + 15 of those 64
     const uint32_t row16 = (uint32_t)(P.TW * 128) >> 4;  // one slab image row, in 16-byte units
-    const uint64_t x_desc0 = gmma_desc(smem_u32(a_ring) + (kPair ? 128u * 128u * wg : 0u));
-    const uint64_t w_desc0 = gmma_desc(smem_u32(b_ring) + (kPair ? 0u : 8192u * wg));
-    constexpr uint32_t A16 = kASlot >> 4, B16 = C::kBSlot >> 4, H16 = 8192u >> 4;
+    const uint64_t x_desc0 = gmma_desc(smem_u32(a_ring));  // paired: both tiles' views, 256 rows
+    const uint64_t w_desc0 = gmma_desc(smem_u32(b_ring) + 8192u * wg);
+    constexpr uint32_t A16 = kASlot >> 4, B16 = C::kBSlot >> 4;
     const int ngroups = P.ngroups, kchunks = P.kchunks;
     int sa = 0, pa = 0, sb = 0, pb = 0;
     const int e = warp - 4;  // 0..7
@@ -227,63 +235,57 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     uint32_t res_par = 0;
     const int cpg = P.gn_cpg;
     const int red = 4 * (cpg < 8 ? cpg : 8);  // lanes holding one GroupNorm group's (channel, pixel) partial sums
-    // first of the 16 channels this warp finishes in half h of the column block at n0
-    auto chan0 = [&](int n0, int h) { return n0 + 64 * (kPair ? h : wg) + 16 * q; };
+    // first of the 16 channels this warp finishes in the column block at n0
+    auto chan0 = [&](int n0) { return n0 + 64 * wg + 16 * q; };
     // norm-backward sums: the "residual" tile is x and is not added
     const bool nb = P.nb_sums != nullptr;
-    // per thread and half: channel c (index 0) and c + 8 (index 1); the sums run on across consecutive items of the
-    // same (image, channel block) and are flushed when that changes.  Their GroupNorm constants are derived again
-    // for every item: held across items, they would cost the paired accumulator 16 registers.
-    float nb_s1[NH][2], nb_s2[NH][2];
-#pragma unroll
-    for (int h = 0; h < NH; ++h)
-#pragma unroll
-      for (int k = 0; k < 2; ++k) nb_s1[h][k] = nb_s2[h][k] = 0.f;
+    // per thread: channel c (index 0) and c + 8 (index 1); the sums run on across consecutive items of the same
+    // (image, channel block) and are flushed when that changes.  Their GroupNorm constants are derived again for
+    // every tile: held across items, they would cost the paired accumulator registers.
+    float nb_s1[2] = {0.f, 0.f}, nb_s2[2] = {0.f, 0.f};
     int nb_img = -1, nb_n0 = -1;
-    // residual (or x) boxes of half h of this warp's tile, into the boxes the previous stores read from
-    auto load_res = [&](const TileCoord& t, int h) {
+    // residual (or x) boxes of this warp's channels of the tile at row h0, into the boxes the previous stores read from
+    auto load_res = [&](const TileCoord& t, int h0) {
       tma_store_wait_read<0>();
       mbar_expect_tx(&res_bar[e], kSwapWarpBuf);
       for (int k = 0; k < 4; ++k)
-        tma_load_4d(&tmR, &res_bar[e], my_buf + k * kSwapBox, chan0(t.n0, h), t.w0, t.h0 + k * rows_per_box, t.img);
+        tma_load_4d(&tmR, &res_bar[e], my_buf + k * kSwapBox, chan0(t.n0), t.w0, h0 + k * rows_per_box, t.img);
     };
 
     for (int tile = tile_first; tile < tile_end; tile += tile_step) {
-      TileCoord t = decode_item<kPair>(P, tile);
-      if (kPair) t.h0 += wg * P.TH;  // this warpgroup's tile of the pair
-      if (has_res && lane == 0) {
-        // half 0's boxes load while the MMAs run; later halves' go to L2 now, so that their loads are L2 hits
-        load_res(t, 0);
+      const TileCoord t = decode_item<kPair>(P, tile);
+      // none of this warpgroup's 64 channels exists: keep the rings' barrier protocol and do nothing else
+      const bool idle = t.n0 + 64 * wg >= P.n_out;
+      if (has_res && !idle && lane == 0) {
+        // the first tile's boxes load while the MMAs run; the second's go to L2 now, so that its load is an L2 hit
+        load_res(t, t.h0);
 #pragma unroll
-        for (int h = 1; h < NH; ++h)
+        for (int h = 1; h < NT; ++h)
           for (int k = 0; k < 4; ++k)
-            tma_prefetch_4d(&tmR, chan0(t.n0, h), t.w0, t.h0 + k * rows_per_box, t.img);
+            tma_prefetch_4d(&tmR, chan0(t.n0), t.w0, t.h0 + h * P.TH + k * rows_per_box, t.img);
         if (nb && tile + tile_step < tile_end) {
           // the NEXT item's x boxes go to L2 now, so that its loads above are L2 hits
-          TileCoord tn = decode_item<kPair>(P, tile + tile_step);
-          if (kPair) tn.h0 += wg * P.TH;
+          const TileCoord tn = decode_item<kPair>(P, tile + tile_step);
 #pragma unroll
-          for (int h = 0; h < NH; ++h)
+          for (int h = 0; h < NT; ++h)
             for (int k = 0; k < 4; ++k)
-              tma_prefetch_4d(&tmR, chan0(tn.n0, h), tn.w0, tn.h0 + k * rows_per_box, tn.img);
+              tma_prefetch_4d(&tmR, chan0(tn.n0), tn.w0, tn.h0 + h * P.TH + k * rows_per_box, tn.img);
         }
       }
-      float acc[NH][64];
-      {
+      float acc[64 * NT];
+      // the item's MMA groups; kIdle: the same waits and releases without the MMAs
+      auto mainloop = [&](auto kIdle) {
         uint32_t accf = 0;
         int rel_b = -1, rel_a = -1;  // the slots the group in flight is the last reader of (-1: none)
         // every consumer thread arrives (a lane-0 arrival between wgmmas puts them on a divergent path, and ptxas
         // then serialises every MMA); the arrivals are for the previous group, which wait_group 1 has completed
         auto group = [&](uint64_t w, uint64_t x, int last_b, int last_a) {
-          wgmma_fence();
-#pragma unroll
-          for (int h = 0; h < NH; ++h) {
-            uint32_t f = accf;
-            wgmma_chunk<0, 0>(acc[h], w + h * H16, x, f);
+          if constexpr (!decltype(kIdle)::value) {
+            wgmma_fence();
+            wgmma_chunk<0, 0>(acc, w, x, accf);
+            wgmma_commit();
+            wgmma_wait<1>();
           }
-          accf = 1;
-          wgmma_commit();
-          wgmma_wait<1>();
           if (rel_b >= 0) mbar_arrive(&b_empty[rel_b]);
           if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
           rel_b = last_b;
@@ -324,55 +326,57 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             }
           }
         }
-        wgmma_wait<0>();
-#pragma unroll
-        for (int h = 0; h < NH; ++h) wgmma_fence_regs(acc[h]);
+        if constexpr (!decltype(kIdle)::value) {
+          wgmma_wait<0>();
+          wgmma_fence_regs(acc);
+        }
         if (rel_b >= 0) mbar_arrive(&b_empty[rel_b]);
         if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
+      };
+      if (idle) {
+        mainloop(std::true_type{});
+        continue;
       }
-      // interior tiles need no per-pixel validity test for the GroupNorm / norm-backward sums
-      const bool interior = (t.h0 + P.TH <= P.H) && (t.w0 + P.TW <= P.W);
-      // bit 2 j + b: this thread's pixel 8 j + m2 + b lies inside the image (one register for both halves)
-      uint32_t ok_mask = ~0u;
-      if (!interior) {
-        ok_mask = 0;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int p = 8 * (j >> 1) + m2 + (j & 1);
-          if ((t.h0 + (p >> tw_shift) < P.H) && (t.w0 + (p & (P.TW - 1)) < P.W)) ok_mask |= 1u << j;
-        }
-      }
-      auto pix_ok = [&](int i) { return ((ok_mask >> (2 * (i >> 2) + (i & 1))) & 1u) != 0; };
+      mainloop(std::false_type{});
       if (nb && (t.img != nb_img || t.n0 != nb_n0)) {  // the previous (image, channel block)'s sums are flushed
+        if (nb_img >= 0)
+          nb_flush(P, nb_img, chan0(nb_n0) + (lane >> 2), lane, nb_s1[0], nb_s1[1], nb_s2[0], nb_s2[1]);
 #pragma unroll
-        for (int h = 0; h < NH; ++h) {
-          if (nb_img >= 0)
-            nb_flush(P, nb_img, chan0(nb_n0, h) + (lane >> 2), lane, nb_s1[h][0], nb_s1[h][1], nb_s2[h][0],
-                     nb_s2[h][1]);
-#pragma unroll
-          for (int k = 0; k < 2; ++k) nb_s1[h][k] = nb_s2[h][k] = 0.f;
-        }
+        for (int k = 0; k < 2; ++k) nb_s1[k] = nb_s2[k] = 0.f;
         nb_img = t.img;
         nb_n0 = t.n0;
       }
+      const int c0 = chan0(t.n0);       // this warp's 16 output channels
+      const int ca = c0 + (lane >> 2);  // this thread's channels, in every tile of the item: ca and ca + 8
+      float bias2[2] = {0.f, 0.f};
+      if (P.bias_mode == T2H_BIAS_COL) {
+        if (ca < P.n_out) bias2[0] = __ldg(P.bias + t.img * P.bias_sn + ca);
+        if (ca + 8 < P.n_out) bias2[1] = __ldg(P.bias + t.img * P.bias_sn + ca + 8);
+      }
+      float gs[2] = {0.f, 0.f}, gss[2] = {0.f, 0.f};  // GroupNorm partial sums over the item's tiles
 #pragma unroll
-      for (int h = 0; h < NH; ++h) {
-        float(&a)[64] = acc[h];
-        const int c0 = chan0(t.n0, h);     // this warp's 16 output channels of the half
-        const int ca = c0 + (lane >> 2);  // this thread's channels: ca and ca + 8
-        if (h > 0 && has_res && lane == 0) load_res(t, h);
+      for (int h = 0; h < NT; ++h) {
+        float* a = acc + 64 * h;
+        const int th0 = t.h0 + h * P.TH;  // first image row of tile h
+        if (h > 0 && has_res && lane == 0) load_res(t, th0);
+        // interior tiles need no per-pixel validity test for the GroupNorm / norm-backward sums
+        const bool interior = (th0 + P.TH <= P.H) && (t.w0 + P.TW <= P.W);
+        // bit 2 j + b: this thread's pixel 8 j + m2 + b of the tile lies inside the image
+        uint32_t ok_mask = ~0u;
+        if (!interior) {
+          ok_mask = 0;
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const int p = 8 * (j >> 1) + m2 + (j & 1);
+            if ((th0 + (p >> tw_shift) < P.H) && (t.w0 + (p & (P.TW - 1)) < P.W)) ok_mask |= 1u << j;
+          }
+        }
+        auto pix_ok = [&](int i) { return ((ok_mask >> (2 * (i >> 2) + (i & 1))) & 1u) != 0; };
         // accumulator element i: channel ca + 8 ((i >> 1) & 1), pixel 8 (i >> 2) + m2 + (i & 1); in-box pixel and
         // channel of the [32][16] box i >> 4
         auto box_off = [&](int i) { return (i >> 4) * kSwapBox + swz64(8 * ((i >> 2) & 3) + m2 + (i & 1), (lane >> 2) + 8 * ((i >> 1) & 1)); };
-        {
-          float bias2[2] = {0.f, 0.f};
-          if (P.bias_mode == T2H_BIAS_COL) {
-            if (ca < P.n_out) bias2[0] = __ldg(P.bias + t.img * P.bias_sn + ca);
-            if (ca + 8 < P.n_out) bias2[1] = __ldg(P.bias + t.img * P.bias_sn + ca + 8);
-          }
 #pragma unroll
-          for (int i = 0; i < 64; ++i) a[i] = a[i] * P.alpha + bias2[(i >> 1) & 1];
-        }
+        for (int i = 0; i < 64; ++i) a[i] = a[i] * P.alpha + bias2[(i >> 1) & 1];
         if (P.act == T2H_ACT_GELU) {
 #pragma unroll
           for (int i = 0; i < 64; ++i) a[i] = gelu_erf(a[i]);
@@ -418,8 +422,8 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 const int k = (i >> 1) & 1;
                 const float xh = (lds_f32(buf_s + box_off(i)) - nb_mean[k]) * nb_rstd[k];
                 const float du = a[i] * act_grad_fast(fmaf(xh, nb_ga[k], nb_be[k]), 1);
-                nb_s1[h][k] += du;
-                nb_s2[h][k] = fmaf(du, xh, nb_s2[h][k]);
+                nb_s1[k] += du;
+                nb_s2[k] = fmaf(du, xh, nb_s2[k]);
               }
             } else {
               const int an = P.nb_act;
@@ -428,8 +432,8 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 const int k = (i >> 1) & 1;
                 const float xh = (lds_f32(buf_s + box_off(i)) - nb_mean[k]) * nb_rstd[k];
                 const float du = a[i] * ((an == 2 && fmaf(xh, nb_ga[k], nb_be[k]) <= 0.f) ? 0.2f : 1.0f);
-                nb_s1[h][k] += du;
-                nb_s2[h][k] = fmaf(du, xh, nb_s2[h][k]);
+                nb_s1[k] += du;
+                nb_s2[k] = fmaf(du, xh, nb_s2[k]);
               }
             }
           } else {
@@ -438,33 +442,11 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           }
         }
         if (P.gn_stats) {
-          float gs[2] = {0.f, 0.f}, gss[2] = {0.f, 0.f};
 #pragma unroll
           for (int i = 0; i < 64; ++i) {
             const float x = (interior || pix_ok(i)) ? a[i] : 0.f;
             gs[(i >> 1) & 1] += x;
             gss[(i >> 1) & 1] = fmaf(x, x, gss[(i >> 1) & 1]);
-          }
-          // lanes 4c .. 4c + 3 hold channel c's pixels; the channels of a group are consecutive lane quads
-          for (int off = 1; off < red; off <<= 1) {
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              gs[k] += __shfl_xor_sync(0xffffffffu, gs[k], off);
-              gss[k] += __shfl_xor_sync(0xffffffffu, gss[k], off);
-            }
-          }
-          if (cpg >= 16) {  // channels ca and ca + 8 are in the same group
-            gs[0] += gs[1];
-            gss[0] += gss[1];
-          }
-          if ((lane & (red - 1)) == 0) {
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              if (k == 1 && cpg >= 16) break;
-              double* dst = P.gn_stats + ((long long)t.img * P.gn_groups + (ca + 8 * k) / cpg) * 2;
-              atomicAdd(dst, (double)gs[k]);
-              atomicAdd(dst + 1, (double)gss[k]);
-            }
           }
         }
         if (P.epi_mode == EPI_DIRECT) {
@@ -474,7 +456,7 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           for (int i = 0; i < 64; ++i) {
             const int c = ca + 8 * ((i >> 1) & 1);
             const int p = 8 * (i >> 2) + m2 + (i & 1);
-            const int hh = t.h0 + (p >> tw_shift), w = t.w0 + (p & (P.TW - 1));
+            const int hh = th0 + (p >> tw_shift), w = t.w0 + (p & (P.TW - 1));
             if (c < P.n_out && hh < P.H && w < P.W) dst[(long long)c * P.d_sc + (long long)hh * P.d_sh + (long long)w * P.d_sw] = a[i];
           }
           continue;
@@ -493,17 +475,37 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           fence_proxy_async_smem();
           __syncwarp();
           if (lane == 0) {
-            tma_store_4d(&tmD, my_buf + k * kSwapBox, c0, t.w0, t.h0 + k * rows_per_box, t.img);
+            tma_store_4d(&tmD, my_buf + k * kSwapBox, c0, t.w0, th0 + k * rows_per_box, t.img);
             tma_store_commit();
           }
         }
       }
-    }
-    if (nb && nb_img >= 0) {
+      if (P.gn_stats) {
+        // lanes 4c .. 4c + 3 hold channel c's pixels; the channels of a group are consecutive lane quads
+        for (int off = 1; off < red; off <<= 1) {
 #pragma unroll
-      for (int h = 0; h < NH; ++h)
-        nb_flush(P, nb_img, chan0(nb_n0, h) + (lane >> 2), lane, nb_s1[h][0], nb_s1[h][1], nb_s2[h][0], nb_s2[h][1]);
+          for (int k = 0; k < 2; ++k) {
+            gs[k] += __shfl_xor_sync(0xffffffffu, gs[k], off);
+            gss[k] += __shfl_xor_sync(0xffffffffu, gss[k], off);
+          }
+        }
+        if (cpg >= 16) {  // channels ca and ca + 8 are in the same group
+          gs[0] += gs[1];
+          gss[0] += gss[1];
+        }
+        if ((lane & (red - 1)) == 0) {
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            if (k == 1 && cpg >= 16) break;
+            double* dst = P.gn_stats + ((long long)t.img * P.gn_groups + (ca + 8 * k) / cpg) * 2;
+            atomicAdd(dst, (double)gs[k]);
+            atomicAdd(dst + 1, (double)gss[k]);
+          }
+        }
+      }
     }
+    if (nb && nb_img >= 0)
+      nb_flush(P, nb_img, chan0(nb_n0) + (lane >> 2), lane, nb_s1[0], nb_s1[1], nb_s2[0], nb_s2[1]);
     if (lane == 0) tma_store_wait_read<0>();
   }
 }
