@@ -1,8 +1,8 @@
 """Every path of the tap-GEMM (t2h_tapgemm) and the GroupNorm statistics kernel, element by element against fp64.
 
 The case table below names the kernel, epilogue, column tile (BN) and spatial tile (TW x TH) each convolution is meant
-to run on, through ``route``: a restatement of the selection rule in csrc/gemm_tc.cu (t2h_tapgemm, "tile shape" to
-"epilogue mode").  It documents intent and does not verify the C code; a change to the routing updates ``route`` in
+to run on, through ``route``: a restatement of the selection rule in csrc/gemm_tc.cu (plan_tapgemm, tile shape to
+epilogue mode).  It documents intent and does not verify the C code; a change to the routing updates ``route`` in
 the same change, and ``test_case_table_covers_every_path`` then says which path or factor level lost its case.
 
 Bounds, shared by every case:

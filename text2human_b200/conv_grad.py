@@ -15,6 +15,8 @@ Kinds:  "k3" 3x3 s1 p1 | "k1" 1x1 | "down" pad (0,1,0,1) + 3x3 s2 (Downsample, v
         "k4s2" 4x4 s2 p1 and "k4s1" 4x4 s1 p1 (Discriminator, :1160-1197).
 Stride-2 kinds take their input as 4-phase space-to-depth planes ``[T, 4, N, H/2, W/2, C]``.
 """
+import functools
+
 import torch
 
 from . import ops
@@ -36,8 +38,9 @@ def out_hw(kind, H, W):
     return H // 2, W // 2          # down, k4s2 (even H, W)
 
 
+@functools.lru_cache(maxsize=None)
 def fwd_taps(kind, n):
-    """((dy, dx, img_off), ...) in weight-slot order kh*K + kw"""
+    """((dy, dx, img_off), ...) in weight-slot order kh*K + kw (cached: every strided conv launch asks for it)"""
     K, pad = KSIZE[kind], PAD[kind]
     taps = []
     for kh in range(K):

@@ -130,6 +130,17 @@ __device__ __forceinline__ TileCoord decode_tile(const TapGemmDev& P, int tile, 
   return t;
 }
 
+// TMA write of one staged fp32 unit (columns c0.., the tile's pixels) of work item `work`
+__device__ __forceinline__ void store_f32_unit(const TapGemmDev& P, const CUtensorMap* tmD, const uint8_t* src, int c0,
+                                               const TileCoord& t, int work) {
+  if (P.partials)  // deterministic split-K: every k-slice owns a slab; a fixed-order pass sums them
+    tma_store_4d(tmD, src, c0, t.w0, t.h0, t.img + work / P.total_tiles);
+  else if (P.ksplit > 1 || P.accum)  // partial sum of a k-slice, or an accumulating launch
+    tma_reduce_add_4d(tmD, src, c0, t.w0, t.h0, t.img);
+  else
+    tma_store_4d(tmD, src, c0, t.w0, t.h0, t.img);
+}
+
 // byte offset of 16-byte chunk j of row r inside a 128B-swizzled [128 rows][128 bytes] tile
 __device__ __forceinline__ int swz(int r, int j) { return r * 128 + ((j ^ (r & 7)) << 4); }
 
@@ -466,13 +477,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             for (int half = 0; half < 2; ++half) {
               const int c0 = col0 + half * 32;
               if (c0 >= P.n_out) break;
-              const uint8_t* ob = o0 + half * kEpiBufBytes;
-              if (P.partials)  // deterministic split-K: every k-slice owns a slab; a fixed-order pass sums them
-                tma_store_4d(&tmD, ob, c0, t.w0, t.h0, t.img + work / P.total_tiles);
-              else if (P.ksplit > 1 || P.accum)
-                tma_reduce_add_4d(&tmD, ob, c0, t.w0, t.h0, t.img);
-              else
-                tma_store_4d(&tmD, ob, c0, t.w0, t.h0, t.img);
+              store_f32_unit(P, &tmD, o0 + half * kEpiBufBytes, c0, t, work);
             }
             tma_store_commit();
             tma_store_wait_read<1>();  // the other pair is free again
@@ -514,16 +519,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               }
             }
           }
-          if (P.act == T2H_ACT_GELU) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
-          } else if (P.act == T2H_ACT_RELU) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-          } else if (P.act == T2H_ACT_LRELU) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = v[i] > 0.f ? v[i] : 0.2f * v[i];
-          }
+          apply_act<32>(v, P.act);
           if (has_res) {
             mbar_wait(&res_bar[buf], (res_par >> buf) & 1);
             res_par ^= 1u << buf;
@@ -554,12 +550,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           fence_proxy_async_smem();
           named_bar_sync(2, 128);  // staging tile complete; residual tile fully consumed
           if (elected) {
-            if (P.partials)  // deterministic split-K: every k-slice owns a slab; a fixed-order pass sums them
-              tma_store_4d(&tmD, ob, col0, t.w0, t.h0, t.img + work / P.total_tiles);
-            else if (P.ksplit > 1 || P.accum)
-              tma_reduce_add_4d(&tmD, ob, col0, t.w0, t.h0, t.img);  // partial sum of a k-slice
-            else
-              tma_store_4d(&tmD, ob, col0, t.w0, t.h0, t.img);
+            store_f32_unit(P, &tmD, ob, col0, t, work);
             tma_store_commit();
             if (has_res && cc + 2 < nuc) issue_res(cc + 2, buf);
             tma_store_wait_read<1>();  // the other staging tile is free again
@@ -619,16 +610,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 v[i] += b4.x; v[i + 1] += b4.y; v[i + 2] += b4.z; v[i + 3] += b4.w;
               }
             }
-            if (P.act == T2H_ACT_GELU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
-            } else if (P.act == T2H_ACT_RELU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-            } else if (P.act == T2H_ACT_LRELU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = v[i] > 0.f ? v[i] : 0.2f * v[i];
-            }
+            apply_act<32>(v, P.act);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
               __align__(16) __half hi[8];
@@ -675,6 +657,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             for (int i = 0; i < CH; ++i)
               if (col0 + i < P.n_out) v[i] += __ldg(P.bias + t.img * P.bias_sn + col0 + i);
           }
+          // written out rather than apply_act<CH>, which changes the instruction schedule of tapgemm_kernel<32>
           if (P.act == T2H_ACT_GELU) {
 #pragma unroll
             for (int i = 0; i < CH; ++i) v[i] = gelu_erf(v[i]);
@@ -776,18 +759,25 @@ static int make_tmap(CUtensorMap* tm, const void* base, int elem_bytes, int rank
   return T2H_OK;
 }
 
+// The kernels take the whole opt-in shared memory; the attribute lives in each device's copy of the function, so it is
+// set once per (kernel, device).
+template <auto kKernel>
+static int allow_full_smem() {
+  static bool configured[64] = {};
+  int dev = 0;
+  T2H_CUDA(cudaGetDevice(&dev));
+  if (!configured[dev & 63]) {
+    T2H_CUDA(cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDynSmem));
+    configured[dev & 63] = true;
+  }
+  return T2H_OK;
+}
+
 template <int BN>
 static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
                   const CUtensorMap& tmR, const TapGemmDev& P, cudaStream_t stream) {
   using C = Cfg<BN>;
-  static bool configured[64] = {};
-  int dev = 0;
-  T2H_CUDA(cudaGetDevice(&dev));
-  if (!configured[dev & 63]) {  // per device: the attribute lives in the device's copy of the function
-    T2H_CUDA(cudaFuncSetAttribute(tapgemm_kernel<BN>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, kDynSmem));
-    configured[dev & 63] = true;
-  }
+  if (int rc = allow_full_smem<tapgemm_kernel<BN>>()) return rc;
   // ring depths: enough bytes in flight to cover the TMA round trip at the tile's consumption rate.
   // With the 3-product split both (hi, lo) slabs of a (group, chunk) are live at once.
   TapGemmDev Q = P;
@@ -806,14 +796,7 @@ template <bool kPair>
 static int launch_swap(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
                        const CUtensorMap& tmR, const TapGemmDev& P, cudaStream_t stream) {
   using C = Cfg<128>;
-  static bool configured[64] = {};
-  int dev = 0;
-  T2H_CUDA(cudaGetDevice(&dev));
-  if (!configured[dev & 63]) {
-    T2H_CUDA(cudaFuncSetAttribute(tapgemm_swap_kernel<kPair>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  kDynSmem));
-    configured[dev & 63] = true;
-  }
+  if (int rc = allow_full_smem<tapgemm_swap_kernel<kPair>>()) return rc;
   TapGemmDev Q = P;
   // ring depths from what the register epilogue leaves of the shared memory.  Unpaired: 4 A slabs load the next
   // chunk's hi and lo slabs during the whole current chunk, the rest holds weight tiles (4: two taps of the 3-product
@@ -827,6 +810,191 @@ static int launch_swap(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
   T2H_CUDA(launch_pdl(tapgemm_swap_kernel<kPair>, dim3(grid), dim3(kSwapThreads), kDynSmem, stream, tmA, tmB, tmD,
                       tmR, Q));
+  return T2H_OK;
+}
+
+enum { KERNEL_GENERIC = 0, KERNEL_SWAP = 1, KERNEL_SWAP_PAIR = 2 };
+
+// What a t2h_tapgemm launch runs on: kernel, spatial tile of one 128-row block (TW x TH output positions of one image),
+// column tile BN and epilogue mode.
+struct TapGemmPlan {
+  int kernel;        // KERNEL_*
+  bool swap_direct;  // swapped kernel with the direct (strided) epilogue
+  int TW, TH, BN, epi_mode;
+};
+
+// (tests/test_gpu_tapgemm_paths.py::route restates this selection, tile shape to epilogue mode, and labels its cases
+// with it: a routing change updates it in the same change)
+static TapGemmPlan plan_tapgemm(const t2h_tapgemm_params* p) {
+  TapGemmPlan L;
+  const bool rows_mode = p->H == 1 || p->tile_rows;
+  if (rows_mode) {
+    L.TW = 128; L.TH = 1;
+  } else {
+    L.TW = 16;
+    while (L.TW > p->W && L.TW > 1) L.TW >>= 1;  // W < 16: narrower, taller boxes
+    L.TH = 128 / L.TW;
+  }
+  // Swapped-operand kernel (gemm_tc_swap.cuh): spatial convs with plain fp32 outputs.  The weight tile is the M
+  // operand, the 128-pixel tile the N operand.  MN-major operands exist only in row GEMMs.
+  const bool swap_any = !rows_mode && !p->a_mn && !p->b_mn && p->d_mode == T2H_OUT_F32 &&
+                        p->bias_mode != T2H_BIAS_ROW && !p->a_bcast && !p->b_batched && !p->b_batched_h;
+  // ... Cout % 128 == 0 and an NHWC destination the TMA epilogue can address
+  const bool swap_tma = swap_any && p->n_out % 128 == 0 && p->d_sc == 1 && p->d_sw % 4 == 0 && p->d_sh % 4 == 0 &&
+                        p->d_sh > 0 && (p->n_img == 1 || (p->d_sn % 4 == 0 && p->d_sn > 0)) &&
+                        reinterpret_cast<uintptr_t>(p->d) % 16 == 0 &&
+                        (!p->residual || reinterpret_cast<uintptr_t>(p->residual) % 16 == 0) &&
+                        (!p->gn_stats ||
+                         (p->gn_cpg >= 1 && (p->gn_cpg & (p->gn_cpg - 1)) == 0 && p->n_out % p->gn_cpg == 0));
+  // ... or small-Cout convs writing NCHW (conv_out) through the direct epilogue: the weight tile is zero-padded to 128
+  // rows by TMA
+  L.swap_direct = swap_any && p->d_sc != 1 && p->n_out <= 128 && !p->residual && !p->gn_stats &&
+                  p->act == T2H_ACT_NONE;
+  const bool swap = swap_tma || L.swap_direct;
+  if (swap) {
+    L.BN = 128;
+  } else {
+    L.BN = 16;
+    while (L.BN < p->n_out && L.BN < 128) L.BN <<= 1;
+    if (p->b_mn && L.BN < 64) L.BN = 64;  // an MN-major B tile is made of whole 64-column boxes
+  }
+  // Paired mode of the swapped kernel: one CTA computes two vertically adjacent tiles that share every weight tile
+  // and one slab, halving the weight bytes per output pixel.  It halves the number of work items too, so it is taken
+  // only when there are still at least as many pairs as SMs.
+  const long long tiles =
+      (long long)p->n_img * ceil_div(p->W, L.TW) * ceil_div(p->H, L.TH) * ceil_div(p->n_out, L.BN);
+  L.kernel = !swap ? KERNEL_GENERIC : (tiles >= 2LL * num_sms() ? KERNEL_SWAP_PAIR : KERNEL_SWAP);
+
+  // the generic kernel's TMA epilogues need a dense, 16-byte aligned output
+  const int align_el = p->d_mode == T2H_OUT_F32 ? 4 : 8;  // elements per 16 bytes
+  bool tma_ok = p->d_sc == 1 && p->n_out % align_el == 0 && p->d_sw % align_el == 0 &&
+                reinterpret_cast<uintptr_t>(p->d) % 16 == 0 && L.BN >= (p->d_mode == T2H_OUT_F32 ? 32 : 64);
+  // strides of the dims the output domain really uses must be TMA-encodable
+  if (p->H > 1) tma_ok = tma_ok && p->d_sh % align_el == 0 && p->d_sh > 0;
+  if (p->n_img > 1) tma_ok = tma_ok && p->d_sn % align_el == 0 && p->d_sn > 0;
+  if (p->d_mode == T2H_OUT_PLANES && p->d_terms == 2) {
+    // the lo plane is addressed as extra images: its distance must be a whole number of d_sn
+    const long long sn = (p->n_img > 1) ? p->d_sn : p->d_plane;
+    tma_ok = tma_ok && sn > 0 && p->d_plane % sn == 0 && p->d_plane % align_el == 0;
+  }
+  if (p->residual) tma_ok = tma_ok && (reinterpret_cast<uintptr_t>(p->residual) % 16 == 0);
+  if (p->bias_mode == T2H_BIAS_COL)
+    tma_ok = tma_ok && (reinterpret_cast<uintptr_t>(p->bias) % 16 == 0) && p->bias_sn % 4 == 0;
+  if (swap)
+    L.epi_mode = L.swap_direct ? EPI_DIRECT : EPI_TMA_F32;
+  else
+    L.epi_mode = !tma_ok ? EPI_DIRECT : (p->d_mode == T2H_OUT_F32 ? EPI_TMA_F32 : EPI_TMA_PLANES);
+  return L;
+}
+
+// Taps with the same (dx, img_off) share one activation slab when a vertical shift of the slab view stays 1024-byte
+// aligned (TW*128 bytes per image row, TW >= 8); a slab then spans TH + (the group's dy range) rows.
+static void group_taps(const t2h_tapgemm_params* p, int TW, int TH, TapGemmDev* P) {
+  const bool can_share = (TW >= 8) && (TW <= 16);
+  P->ngroups = 0;
+  int gmin[T2H_MAX_TAPS], gmax[T2H_MAX_TAPS];
+  int gt_dy[T2H_MAX_TAPS][3];
+  for (int i = 0; i < p->ntaps; ++i) {
+    int g = -1;
+    if (can_share)
+      for (int k = 0; k < P->ngroups; ++k)
+        if (P->g_dx[k] == p->tap_dx[i] && P->g_ioff[k] == p->tap_img_off[i] && P->g_ntaps[k] < 3) {
+          const int lo = p->tap_dy[i] < gmin[k] ? p->tap_dy[i] : gmin[k];
+          const int hi = p->tap_dy[i] > gmax[k] ? p->tap_dy[i] : gmax[k];
+          if (hi - lo <= 2) { g = k; gmin[k] = lo; gmax[k] = hi; break; }
+        }
+    if (g < 0) {
+      g = P->ngroups++;
+      P->g_dx[g] = p->tap_dx[i]; P->g_ioff[g] = p->tap_img_off[i]; P->g_ntaps[g] = 0;
+      gmin[g] = gmax[g] = p->tap_dy[i];
+    }
+    gt_dy[g][P->g_ntaps[g]] = p->tap_dy[i];
+    P->g_btap[g][P->g_ntaps[g]] = p->use_tap_w ? p->tap_w[i] : i;
+    P->g_ntaps[g]++;
+  }
+  int extra = 0;
+  for (int g = 0; g < P->ngroups; ++g) {
+    P->g_dy0[g] = gmin[g];
+    for (int k = 0; k < P->g_ntaps[g]; ++k) P->g_dyrel[g][k] = gt_dy[g][k] - gmin[g];
+    if (gmax[g] - gmin[g] > extra) extra = gmax[g] - gmin[g];
+  }
+  for (int g = P->ngroups; g < T2H_MAX_TAPS; ++g) {
+    P->g_dx[g] = P->g_ioff[g] = P->g_dy0[g] = P->g_ntaps[g] = 0;
+  }
+  P->slab_rows = TH + extra;
+}
+
+// split-K: ks k-slices of kchunks contraction chunks, clamped to [1, kchunks]; the last slice may be shorter, so
+// fewer slices than requested can come out (ops.split_slices restates this count)
+static void set_k_slices(TapGemmDev& P, int ks) {
+  if (ks < 1) ks = 1;
+  if (ks > P.kchunks) ks = P.kchunks;
+  P.kper = ceil_div(P.kchunks, ks);
+  P.ksplit = ceil_div(P.kchunks, P.kper);
+}
+
+// tensor maps of A, B, D and the residual for a planned launch (tmD / tmR are unused copies of tmA on the direct
+// epilogue); sets P.d_term_imgs, the image offset of the lo output plane
+static int encode_tapgemm_maps(const t2h_tapgemm_params* p, const TapGemmPlan& L, TapGemmDev& P, CUtensorMap* tmA,
+                               CUtensorMap* tmB, CUtensorMap* tmD, CUtensorMap* tmR) {
+  {
+    uint64_t dims[4] = {(uint64_t)p->C, (uint64_t)p->a_W, (uint64_t)p->a_H, (uint64_t)p->a_imgs};
+    uint64_t str[4] = {1, (uint64_t)p->a_sw, (uint64_t)p->a_sh, (uint64_t)p->a_sn};
+    uint32_t box[4] = {(uint32_t)kBK, (uint32_t)L.TW, (uint32_t)P.slab_rows, 1};
+    if (p->a_mn) {  // (row, k, h, img): rows contiguous, a_sw = distance between consecutive k
+      dims[0] = (uint64_t)p->a_W; dims[1] = (uint64_t)p->C;
+      box[0] = 64; box[1] = (uint32_t)kBK; box[2] = 1;
+    }
+    int rc = make_tmap(tmA, p->a, 2, 4, dims, str, box, "tapgemm A");
+    if (rc) return rc;
+  }
+  {
+    const int g2 = p->b_groups2 > 0 ? p->b_groups2 : 1;
+    uint64_t dims[4] = {(uint64_t)p->C, (uint64_t)p->n_out, (uint64_t)p->b_groups, (uint64_t)g2};
+    uint64_t str[4] = {1, (uint64_t)p->b_sn, (uint64_t)p->b_sg,
+                       (uint64_t)(g2 > 1 ? p->b_sg2 : p->b_sg)};
+    uint32_t box[4] = {(uint32_t)kBK, (uint32_t)L.BN, 1, 1};
+    if (p->b_mn) {  // (n, k, g, g2): output columns contiguous, b_sn = distance between consecutive k
+      dims[0] = (uint64_t)p->n_out; dims[1] = (uint64_t)p->C;
+      box[0] = 64; box[1] = (uint32_t)kBK;
+    }
+    int rc = make_tmap(tmB, p->b, 2, 4, dims, str, box, "tapgemm B");
+    if (rc) return rc;
+  }
+  *tmD = *tmA;
+  *tmR = *tmA;
+  if (L.epi_mode == EPI_DIRECT) return T2H_OK;
+  // dims the output domain does not use get a harmless, 16-byte-aligned stride
+  const int esz = (p->d_mode == T2H_OUT_F32) ? 4 : 2;
+  const uint64_t sw = (uint64_t)p->d_sw;
+  const uint64_t sh = (p->H > 1) ? (uint64_t)p->d_sh : sw * (uint64_t)p->W;
+  uint64_t sn = (p->n_img > 1) ? (uint64_t)p->d_sn : sh * (uint64_t)p->H;
+  uint64_t imgs = (uint64_t)p->n_img;
+  if (P.partials) {  // one slab per k-slice, addressed through the image dim
+    sn = (uint64_t)p->d_slab;
+    imgs = (uint64_t)P.ksplit;
+  }
+  if (L.epi_mode == EPI_TMA_PLANES && p->d_terms == 2) {
+    if (p->n_img == 1) sn = (uint64_t)p->d_plane;
+    P.d_term_imgs = (int)(p->d_plane / (long long)sn);
+    imgs = (uint64_t)P.d_term_imgs + (uint64_t)p->n_img;
+  }
+  uint64_t dims[4] = {(uint64_t)p->n_out, (uint64_t)p->W, (uint64_t)p->H, imgs};
+  uint64_t str[4] = {1, sw, sh, sn};
+  uint32_t box[4] = {(uint32_t)(esz == 4 ? 32 : 64), (uint32_t)L.TW, (uint32_t)L.TH, 1};
+  CUtensorMapSwizzle sw_mode = CU_TENSOR_MAP_SWIZZLE_128B;
+  if (L.kernel != KERNEL_GENERIC) {  // one box of a swapped-kernel warp: 16 channels (64 bytes) x 32 pixels
+    box[0] = 16;
+    box[2] = (uint32_t)(32 / L.TW);
+    sw_mode = CU_TENSOR_MAP_SWIZZLE_64B;
+  }
+  int rc = make_tmap(tmD, p->d, esz, 4, dims, str, box, "tapgemm D", sw_mode);
+  if (rc) return rc;
+  if (p->residual) {
+    uint64_t rdims[4] = {(uint64_t)p->n_out, (uint64_t)p->W, (uint64_t)p->H, (uint64_t)p->n_img};
+    rc = make_tmap(tmR, p->residual, 4, 4, rdims, str, box, "tapgemm residual", sw_mode);
+    if (rc) return rc;
+  }
   return T2H_OK;
 }
 
@@ -863,7 +1031,12 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
                 "tapgemm: residual add needs fp32 output");
   T2H_CHECK_ARG(p->bias_mode == T2H_BIAS_NONE || p->bias != nullptr, "tapgemm: bias_mode without bias");
   T2H_CHECK_ARG(!p->b_batched_h || p->H == 1 || p->tile_rows, "tapgemm: b_batched_h needs row tiles");
+  T2H_CHECK_ARG(!(p->a_mn || p->b_mn) ||
+                    ((p->H == 1 || p->tile_rows) && p->ntaps == 1 && p->tap_dx[0] == 0 && p->tap_dy[0] == 0),
+                "tapgemm: a_mn / b_mn operands need a row GEMM (H == 1 or tile_rows) with one tap");
 
+  const TapGemmPlan L = plan_tapgemm(p);
+  const bool swap = L.kernel != KERNEL_GENERIC;
   TapGemmDev P;
   memset(&P, 0, sizeof(P));
   P.n_img = p->n_img; P.H = p->H; P.W = p->W;
@@ -879,142 +1052,41 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
   P.nb_eps = p->nb_eps; P.nb_act = p->nb_act; P.nb_groups = p->nb_groups;
   P.n_major = p->nb_sums ? 1 : 0;
   P.gn_groups = p->gn_cpg > 0 ? p->n_out / p->gn_cpg : 0;
-  P.d_term_imgs = 0;
+  P.TW = L.TW; P.TH = L.TH; P.epi_mode = L.epi_mode;
 
-  // ---- tile shape
-  // (tests/test_gpu_tapgemm_paths.py::route restates the selection below, tile shape to epilogue mode, and labels its
-  // cases with it: a routing change updates it in the same change)
-  // one 128-row block = TH x TW output positions of one image
-  int TW, TH;
-  if (p->H == 1 || p->tile_rows) {
-    TW = 128; TH = 1;
-  } else {
-    TW = 16;
-    while (TW > p->W && TW > 1) TW >>= 1;  // W < 16: narrower, taller boxes
-    TH = 128 / TW;
-  }
-  // Swapped-operand kernel (gemm_tc_swap.cuh): spatial convs with Cout % 128 == 0 and a plain fp32
-  // NHWC destination.  The weight tile is the M operand, the 128-pixel tile the N operand.
-  const bool rows_mode = (p->H == 1 || p->tile_rows);
-  bool swap = !rows_mode && TW <= 16 && p->n_out % 128 == 0 && p->d_mode == T2H_OUT_F32 && p->d_sc == 1 &&
-              p->bias_mode != T2H_BIAS_ROW && !p->a_bcast && !p->b_batched && !p->b_batched_h &&
-              p->d_sw % 4 == 0 && p->d_sh % 4 == 0 && p->d_sh > 0 && (p->n_img == 1 || (p->d_sn % 4 == 0 && p->d_sn > 0)) &&
-              reinterpret_cast<uintptr_t>(p->d) % 16 == 0 &&
-              (!p->residual || reinterpret_cast<uintptr_t>(p->residual) % 16 == 0) &&
-              (!p->gn_stats || (p->gn_cpg >= 1 && (p->gn_cpg & (p->gn_cpg - 1)) == 0 && p->n_out % p->gn_cpg == 0));
-  // ... and with a direct (strided) epilogue for small-Cout convs writing NCHW (conv_out): the weight
-  // tile is zero-padded to 128 rows by TMA.
-  const bool swap_direct = !swap && !rows_mode && TW <= 16 && p->n_out <= 128 && p->d_mode == T2H_OUT_F32 &&
-                           p->d_sc != 1 && p->bias_mode != T2H_BIAS_ROW && !p->a_bcast && !p->b_batched &&
-                           !p->b_batched_h && !p->residual && !p->gn_stats && p->act == T2H_ACT_NONE;
-  if (swap_direct) swap = true;
-  if (p->a_mn || p->b_mn) {
-    T2H_CHECK_ARG(rows_mode && p->ntaps == 1 && p->tap_dx[0] == 0 && p->tap_dy[0] == 0,
-                  "tapgemm: a_mn / b_mn operands need a row GEMM (H == 1 or tile_rows) with one tap");
-    swap = false;
-  }
-  int BN = 16;
-  while (BN < p->n_out && BN < 128) BN <<= 1;
-  if (p->b_mn && BN < 64) BN = 64;  // an MN-major B tile is made of whole 64-column boxes
-  if (swap) BN = 128;
-  P.TW = TW; P.TH = TH;
-  // ---- tap groups: taps with the same (dx, img_off) share one activation slab when a vertical
-  // shift of the slab view stays 1024-byte aligned (TW*128 bytes per image row, TW >= 8)
-  {
-    const bool can_share = (TW >= 8) && (TW <= 16);
-    P.ngroups = 0;
-    int gmin[T2H_MAX_TAPS], gmax[T2H_MAX_TAPS];
-    int gt_dy[T2H_MAX_TAPS][3];
-    for (int i = 0; i < p->ntaps; ++i) {
-      int g = -1;
-      if (can_share)
-        for (int k = 0; k < P.ngroups; ++k)
-          if (P.g_dx[k] == p->tap_dx[i] && P.g_ioff[k] == p->tap_img_off[i] && P.g_ntaps[k] < 3) {
-            const int lo = p->tap_dy[i] < gmin[k] ? p->tap_dy[i] : gmin[k];
-            const int hi = p->tap_dy[i] > gmax[k] ? p->tap_dy[i] : gmax[k];
-            if (hi - lo <= 2) { g = k; gmin[k] = lo; gmax[k] = hi; break; }
-          }
-      if (g < 0) {
-        g = P.ngroups++;
-        P.g_dx[g] = p->tap_dx[i]; P.g_ioff[g] = p->tap_img_off[i]; P.g_ntaps[g] = 0;
-        gmin[g] = gmax[g] = p->tap_dy[i];
-      }
-      gt_dy[g][P.g_ntaps[g]] = p->tap_dy[i];
-      P.g_btap[g][P.g_ntaps[g]] = p->use_tap_w ? p->tap_w[i] : i;
-      P.g_ntaps[g]++;
-    }
-    int extra = 0;
-    for (int g = 0; g < P.ngroups; ++g) {
-      P.g_dy0[g] = gmin[g];
-      for (int k = 0; k < P.g_ntaps[g]; ++k) P.g_dyrel[g][k] = gt_dy[g][k] - gmin[g];
-      if (gmax[g] - gmin[g] > extra) extra = gmax[g] - gmin[g];
-    }
-    for (int g = P.ngroups; g < T2H_MAX_TAPS; ++g) {
-      P.g_dx[g] = P.g_ioff[g] = P.g_dy0[g] = P.g_ntaps[g] = 0;
-    }
-    P.slab_rows = TH + extra;
-  }
-  P.tiles_w = ceil_div(p->W, TW);
-  P.tiles_h = ceil_div(p->H, TH);
-  P.n_tiles_n = ceil_div(p->n_out, BN);
-  long long total = (long long)p->n_img * P.tiles_w * P.tiles_h * P.n_tiles_n;
-  T2H_CHECK_ARG(total < (1LL << 31), "tapgemm: too many tiles");
-  P.total_tiles = (int)total;
-  // Paired mode of the swapped kernel: one CTA computes two vertically adjacent tiles that share every weight tile
-  // and one slab, halving the weight bytes per output pixel.  It halves the number of work items too, so it is taken
-  // only when there are still at least as many pairs as SMs.  P.tiles_h then counts pairs of tile rows.
-  const bool pair = swap && P.total_tiles >= 2 * num_sms();
-  if (pair) {
-    P.slab_rows += TH;
-    T2H_CHECK_ARG(P.slab_rows * TW * 128 <= kSwapPairASlot, "tapgemm: paired slab of %d rows does not fit",
+  group_taps(p, L.TW, L.TH, &P);
+  P.tiles_w = ceil_div(p->W, L.TW);
+  P.n_tiles_n = ceil_div(p->n_out, L.BN);
+  const int row_tiles = ceil_div(p->H, L.TH);
+  T2H_CHECK_ARG((long long)p->n_img * P.tiles_w * row_tiles * P.n_tiles_n < (1LL << 31), "tapgemm: too many tiles");
+  P.tiles_h = row_tiles;
+  if (L.kernel == KERNEL_SWAP_PAIR) {  // a work item is a pair of vertically adjacent tiles on one taller slab
+    P.tiles_h = ceil_div(row_tiles, 2);
+    P.slab_rows += L.TH;
+    T2H_CHECK_ARG(P.slab_rows * L.TW * 128 <= kSwapPairASlot, "tapgemm: paired slab of %d rows does not fit",
                   P.slab_rows);
-    P.tiles_h = ceil_div(P.tiles_h, 2);
-    P.total_tiles = p->n_img * P.tiles_w * P.tiles_h * P.n_tiles_n;
   }
+  P.total_tiles = p->n_img * P.tiles_w * P.tiles_h * P.n_tiles_n;
 
-  // ---- epilogue mode
-  const int esz = (p->d_mode == T2H_OUT_F32) ? 4 : 2;
-  const int align_el = 16 / esz;  // elements per 16 bytes
-  bool tma_ok = p->d_sc == 1 && p->n_out % (p->d_mode == T2H_OUT_F32 ? 4 : 8) == 0 &&
-                p->d_sw % align_el == 0 && (reinterpret_cast<uintptr_t>(p->d) % 16 == 0) &&
-                BN >= (p->d_mode == T2H_OUT_F32 ? 32 : 64);
-  // strides of the dims the output domain really uses must be TMA-encodable
-  if (p->H > 1) tma_ok = tma_ok && p->d_sh % align_el == 0 && p->d_sh > 0;
-  if (p->n_img > 1) tma_ok = tma_ok && p->d_sn % align_el == 0 && p->d_sn > 0;
-  if (p->d_mode == T2H_OUT_PLANES && p->d_terms == 2) {
-    // the lo plane is addressed as extra images: its distance must be a whole number of d_sn
-    const long long sn = (p->n_img > 1) ? p->d_sn : p->d_plane;
-    tma_ok = tma_ok && sn > 0 && p->d_plane % sn == 0 && p->d_plane % align_el == 0;
-  }
-  if (p->residual) tma_ok = tma_ok && (reinterpret_cast<uintptr_t>(p->residual) % 16 == 0);
-  if (p->bias_mode == T2H_BIAS_COL)
-    tma_ok = tma_ok && (reinterpret_cast<uintptr_t>(p->bias) % 16 == 0) && p->bias_sn % 4 == 0;
-  P.epi_mode = !tma_ok ? EPI_DIRECT : (p->d_mode == T2H_OUT_F32 ? EPI_TMA_F32 : EPI_TMA_PLANES);
-  if (swap) P.epi_mode = swap_direct ? EPI_DIRECT : EPI_TMA_F32;
   if (p->nb_sums) {
-    T2H_CHECK_ARG(swap && !swap_direct && p->residual && p->nb_stats && p->nb_gamma && p->nb_beta && !p->gn_stats &&
+    T2H_CHECK_ARG(swap && !L.swap_direct && p->residual && p->nb_stats && p->nb_gamma && p->nb_beta && !p->gn_stats &&
                       p->act == T2H_ACT_NONE && p->nb_act >= 0 && p->nb_act <= 2 && p->nb_groups > 0 &&
                       p->n_out % p->nb_groups == 0 && p->k_split <= 1 && !p->accumulate && !p->k_partials,
                   "tapgemm: nb_sums needs a swapped-kernel conv (n_out %% 128 == 0, fp32 NHWC output), x in `residual`, "
                   "statistics / gamma / beta, and no other epilogue work");
   }
   // ---- split-K: k-slices of one tile go to different CTAs and are reduce-added into a zeroed output
-  P.ksplit = 1;
-  P.kper = P.kchunks;
+  set_k_slices(P, 1);
   if (p->k_partials > 1) {
     T2H_CHECK_ARG(!swap && P.epi_mode == EPI_TMA_F32 && !p->residual && p->bias_mode == T2H_BIAS_NONE &&
                       p->act == T2H_ACT_NONE && !p->gn_stats && p->n_img == 1 && p->k_split <= 1 &&
                       p->d_slab > 0 && p->d_slab % 4 == 0,
                   "tapgemm: k_partials needs a plain single-image fp32 GEMM output and an aligned slab stride");
-    int ks = p->k_partials < P.kchunks ? p->k_partials : P.kchunks;
-    P.kper = ceil_div(P.kchunks, ks);
-    P.ksplit = ceil_div(P.kchunks, P.kper);
+    set_k_slices(P, p->k_partials);
     P.partials = 1;
   } else if (p->k_split > 1 && !swap && P.epi_mode == EPI_TMA_F32 && !p->residual && p->bias_mode != T2H_BIAS_ROW &&
       p->act == T2H_ACT_NONE && !p->gn_stats) {
-    int ks = p->k_split < P.kchunks ? p->k_split : P.kchunks;
-    P.kper = ceil_div(P.kchunks, ks);
-    P.ksplit = ceil_div(P.kchunks, P.kper);
+    set_k_slices(P, p->k_split);
   } else {
     T2H_CHECK_ARG(p->k_split <= 1, "tapgemm: k_split needs an aligned fp32 output and no row bias/act/residual");
   }
@@ -1030,73 +1102,17 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
     T2H_CHECK_ARG(P.epi_mode == EPI_TMA_F32, "tapgemm: gn_stats needs an aligned fp32 NHWC output");
     T2H_CHECK_ARG(p->gn_cpg >= 2 && (p->gn_cpg & (p->gn_cpg - 1)) == 0 && p->n_out % p->gn_cpg == 0,
                   "tapgemm: gn_cpg=%d must be a power of two >= 2 dividing n_out", p->gn_cpg);
-    T2H_CHECK_ARG(BN % p->gn_cpg == 0 || p->n_out <= BN, "tapgemm: group straddles column tiles");
+    T2H_CHECK_ARG(L.BN % p->gn_cpg == 0 || p->n_out <= L.BN, "tapgemm: group straddles column tiles");
   }
 
-  // ---- tensor maps
   CUtensorMap tmA, tmB, tmD, tmR;
-  {
-    uint64_t dims[4] = {(uint64_t)p->C, (uint64_t)p->a_W, (uint64_t)p->a_H, (uint64_t)p->a_imgs};
-    uint64_t str[4] = {1, (uint64_t)p->a_sw, (uint64_t)p->a_sh, (uint64_t)p->a_sn};
-    uint32_t box[4] = {(uint32_t)kBK, (uint32_t)TW, (uint32_t)P.slab_rows, 1};
-    if (p->a_mn) {  // (row, k, h, img): rows contiguous, a_sw = distance between consecutive k
-      dims[0] = (uint64_t)p->a_W; dims[1] = (uint64_t)p->C;
-      box[0] = 64; box[1] = (uint32_t)kBK; box[2] = 1;
-    }
-    int rc = make_tmap(&tmA, p->a, 2, 4, dims, str, box, "tapgemm A");
-    if (rc) return rc;
-  }
-  {
-    const int g2 = p->b_groups2 > 0 ? p->b_groups2 : 1;
-    uint64_t dims[4] = {(uint64_t)p->C, (uint64_t)p->n_out, (uint64_t)p->b_groups, (uint64_t)g2};
-    uint64_t str[4] = {1, (uint64_t)p->b_sn, (uint64_t)p->b_sg,
-                       (uint64_t)(g2 > 1 ? p->b_sg2 : p->b_sg)};
-    uint32_t box[4] = {(uint32_t)kBK, (uint32_t)BN, 1, 1};
-    if (p->b_mn) {  // (n, k, g, g2): output columns contiguous, b_sn = distance between consecutive k
-      dims[0] = (uint64_t)p->n_out; dims[1] = (uint64_t)p->C;
-      box[0] = 64; box[1] = (uint32_t)kBK;
-    }
-    int rc = make_tmap(&tmB, p->b, 2, 4, dims, str, box, "tapgemm B");
-    if (rc) return rc;
-  }
-  tmD = tmA;
-  tmR = tmA;
-  if (P.epi_mode != EPI_DIRECT) {
-    // dims the output domain does not use get a harmless, 16-byte-aligned stride
-    const uint64_t sw = (uint64_t)p->d_sw;
-    const uint64_t sh = (p->H > 1) ? (uint64_t)p->d_sh : sw * (uint64_t)p->W;
-    uint64_t sn = (p->n_img > 1) ? (uint64_t)p->d_sn : sh * (uint64_t)p->H;
-    uint64_t imgs = (uint64_t)p->n_img;
-    if (P.partials) {  // one slab per k-slice, addressed through the image dim
-      sn = (uint64_t)p->d_slab;
-      imgs = (uint64_t)P.ksplit;
-    }
-    if (P.epi_mode == EPI_TMA_PLANES && p->d_terms == 2) {
-      if (p->n_img == 1) sn = (uint64_t)p->d_plane;
-      P.d_term_imgs = (int)(p->d_plane / (long long)sn);
-      imgs = (uint64_t)P.d_term_imgs + (uint64_t)p->n_img;
-    }
-    uint64_t dims[4] = {(uint64_t)p->n_out, (uint64_t)p->W, (uint64_t)p->H, imgs};
-    uint64_t str[4] = {1, sw, sh, sn};
-    uint32_t box[4] = {(uint32_t)(esz == 4 ? 32 : 64), (uint32_t)TW, (uint32_t)TH, 1};
-    CUtensorMapSwizzle sw_mode = CU_TENSOR_MAP_SWIZZLE_128B;
-    if (swap) {  // one box of a swapped-kernel warp: 16 channels (64 bytes) x 32 pixels
-      box[0] = 16;
-      box[2] = (uint32_t)(32 / TW);
-      sw_mode = CU_TENSOR_MAP_SWIZZLE_64B;
-    }
-    int rc = make_tmap(&tmD, p->d, esz, 4, dims, str, box, "tapgemm D", sw_mode);
-    if (rc) return rc;
-    if (p->residual) {
-      uint64_t rdims[4] = {(uint64_t)p->n_out, (uint64_t)p->W, (uint64_t)p->H, (uint64_t)p->n_img};
-      rc = make_tmap(&tmR, p->residual, 4, 4, rdims, str, box, "tapgemm residual", sw_mode);
-      if (rc) return rc;
-    }
-  }
-
+  if (int rc = encode_tapgemm_maps(p, L, P, &tmA, &tmB, &tmD, &tmR)) return rc;
   cudaStream_t s = as_stream(stream);
-  if (swap) return pair ? launch_swap<true>(tmA, tmB, tmD, tmR, P, s) : launch_swap<false>(tmA, tmB, tmD, tmR, P, s);
-  switch (BN) {
+  switch (L.kernel) {
+    case KERNEL_SWAP_PAIR: return launch_swap<true>(tmA, tmB, tmD, tmR, P, s);
+    case KERNEL_SWAP: return launch_swap<false>(tmA, tmB, tmD, tmR, P, s);
+  }
+  switch (L.BN) {
     case 16: return launch<16>(tmA, tmB, tmD, tmR, P, s);
     case 32: return launch<32>(tmA, tmB, tmD, tmR, P, s);
     case 64: return launch<64>(tmA, tmB, tmD, tmR, P, s);
@@ -1149,11 +1165,7 @@ extern "C" int t2h_conv_wgrad(const t2h_conv_wgrad_params* p, t2h_stream_t strea
   P.n_tiles_n = ceil_div(p->cin, BN);
   P.total_tiles = P.n_img * P.tiles_w * P.n_tiles_n;
   P.epi_mode = EPI_TMA_F32;
-  int ks = p->k_split > 0 ? p->k_split : num_sms() / P.total_tiles;
-  if (ks < 1) ks = 1;
-  if (ks > P.kchunks) ks = P.kchunks;
-  P.kper = ceil_div(P.kchunks, ks);
-  P.ksplit = ceil_div(P.kchunks, P.kper);
+  set_k_slices(P, p->k_split > 0 ? p->k_split : num_sms() / P.total_tiles);
   T2H_CHECK_ARG((long long)P.total_tiles * P.ksplit < (1LL << 31), "conv_wgrad: too many work items");
   P.total_work = P.total_tiles * P.ksplit;
 

@@ -377,16 +377,7 @@ tapgemm_swap_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         auto box_off = [&](int i) { return (i >> 4) * kSwapBox + swz64(8 * ((i >> 2) & 3) + m2 + (i & 1), (lane >> 2) + 8 * ((i >> 1) & 1)); };
 #pragma unroll
         for (int i = 0; i < 64; ++i) a[i] = a[i] * P.alpha + bias2[(i >> 1) & 1];
-        if (P.act == T2H_ACT_GELU) {
-#pragma unroll
-          for (int i = 0; i < 64; ++i) a[i] = gelu_erf(a[i]);
-        } else if (P.act == T2H_ACT_RELU) {
-#pragma unroll
-          for (int i = 0; i < 64; ++i) a[i] = fmaxf(a[i], 0.f);
-        } else if (P.act == T2H_ACT_LRELU) {
-#pragma unroll
-          for (int i = 0; i < 64; ++i) a[i] = a[i] > 0.f ? a[i] : 0.2f * a[i];
-        }
+        apply_act<64>(a, P.act);
         if (has_res) {
           mbar_wait(&res_bar[e], res_par);
           res_par ^= 1;

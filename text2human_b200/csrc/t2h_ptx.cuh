@@ -349,6 +349,20 @@ __device__ __forceinline__ float gelu_erf(float x) {
   const float c = p * t * e;  // erfc(|z|)
   return 0.5f * x * (x >= 0.f ? 2.0f - c : c);
 }
+// the tap-GEMM epilogue's activation (T2H_ACT_*) on N values in place; act is launch-uniform
+template <int N>
+__device__ __forceinline__ void apply_act(float* v, int act) {
+  if (act == T2H_ACT_GELU) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) v[i] = gelu_erf(v[i]);
+  } else if (act == T2H_ACT_RELU) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) v[i] = fmaxf(v[i], 0.f);
+  } else if (act == T2H_ACT_LRELU) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) v[i] = v[i] > 0.f ? v[i] : 0.2f * v[i];
+  }
+}
 // derivative of the activation that follows a norm, as a function of the pre-activation u (act: 0 none,
 // 1 swish = u*sigmoid(u), 2 LeakyReLU(0.2)); shared by t2h_norm_bwd's kernels and the conv epilogue that fuses its
 // first pass

@@ -150,17 +150,21 @@ def _tapgemm(*, a, a_term_imgs, a_imgs, a_bcast, n_img, H, W, a_H, a_W, Cc, a_sw
         p.use_tap_w = 1
         for i, wi in enumerate(tap_w):
             p.tap_w[i] = wi
+    _launch(lib.t2h_tapgemm, p, 2.0 * n_img * H * W * n_out * Cc * len(taps), (n_img, H, W, n_out, Cc * len(taps)))
+
+
+def _launch(fn, p, algo, shape):
+    """count one launch of ``fn(p)``; with profile_tapgemm on, bracket it with CUDA events and record it"""
     _count()
-    if _PROFILE["on"]:
-        e0 = torch.cuda.Event(enable_timing=True)
-        e1 = torch.cuda.Event(enable_timing=True)
-        e0.record()
-        _lib.check(lib.t2h_tapgemm(C.byref(p), _stream()))
-        e1.record()
-        algo = 2.0 * n_img * H * W * n_out * Cc * len(taps)
-        _PROFILE["records"].append((algo, algo * p.nterms, e0, e1, (n_img, H, W, n_out, Cc * len(taps))))
+    if not _PROFILE["on"]:
+        _lib.check(fn(C.byref(p), _stream()))
         return
-    _lib.check(lib.t2h_tapgemm(C.byref(p), _stream()))
+    e0 = torch.cuda.Event(enable_timing=True)
+    e1 = torch.cuda.Event(enable_timing=True)
+    e0.record()
+    _lib.check(fn(C.byref(p), _stream()))
+    e1.record()
+    _PROFILE["records"].append((algo, algo * p.nterms, e0, e1, shape))
 
 
 def _alloc_out(shape, planes, terms, device):
@@ -222,28 +226,10 @@ def conv3x3(a, w, bias, *, residual=None, planes_out=False, nchw_out=False, want
     a: planes [T,N,H,W,C]; w: packed planes [T,ntaps,Cout,C] (see pack_conv_weight); bias fp32 [Cout].
     Returns fp32 NHWC [N,H,W,Cout] (or NCHW with nchw_out) or planes [T,N,H,W,Cout]; with
     want_stats also the fused GroupNorm statistics of the fp32 output (or None if not applicable)."""
-    _need_cuda(a, w)
-    T, N, H, W, Cc = a.shape
-    Cout = w.shape[2]
     taps = taps if taps is not None else _TAPS_3x3
-    assert w.shape[1] == len(taps) and w.shape[3] == Cc, (a.shape, w.shape)
-    stats, cpg = _stats_for(Cout, N, a.device, want_stats and not planes_out and not nchw_out)
-    if nchw_out:
-        out = torch.empty((N, Cout, H, W), dtype=torch.float32, device=a.device)
-        d_strides = (Cout * H * W, W, 1, H * W)
-    else:
-        out = _alloc_out((N, H, W, Cout), planes_out, T, a.device)
-        d_strides = (H * W * Cout, W * Cout, Cout, 1)
-    _tapgemm(a=a, a_term_imgs=N, a_imgs=T * N, a_bcast=0, n_img=N, H=H, W=W, a_H=H, a_W=W, Cc=Cc,
-             a_sw=Cc, a_sh=W * Cc, a_sn=H * W * Cc,
-             b=w, b_term_g=len(taps), b_groups=w.shape[0] * len(taps), b_batched=0, n_out=Cout, b_sn=Cc,
-             b_sg=Cout * Cc,
-             taps=taps, d=out, d_mode=OUT_PLANES if planes_out else OUT_F32, d_strides=d_strides,
-             d_plane=N * H * W * Cout, bias=bias, bias_mode=BIAS_COL, residual=residual,
-             gn_stats=stats, gn_cpg=cpg, act=act)
-    if want_stats:
-        return out, stats
-    return out
+    assert w.shape[1] == len(taps), (a.shape, w.shape)
+    return tap_conv(a, w, bias, taps, n=a.shape[1], out_hw=a.shape[2:4], residual=residual, planes_out=planes_out,
+                    nchw_out=nchw_out, want_stats=want_stats, act=act)
 
 
 def pack_upsample_conv_weight(w, terms):
@@ -310,21 +296,10 @@ def conv1x1(a, w, bias, *, residual=None, planes_out=False, want_stats=False):
 def conv3x3_s2(a_ph, w, bias, *, want_stats=False):
     """Downsample conv: pad (0,1,0,1) then 3x3 stride 2 (vqgan_arch.py:547-551).
     a_ph: space-to-depth planes [T,4,N,Ho,Wo,C] from f32_to_planes(mode=S2D)."""
-    _need_cuda(a_ph, w)
+    from .conv_grad import fwd_taps  # conv_grad imports this module
     T, four, N, Ho, Wo, Cc = a_ph.shape
     assert four == 4
-    Cout = w.shape[2]
-    out = torch.empty((N, Ho, Wo, Cout), dtype=torch.float32, device=a_ph.device)
-    stats, cpg = _stats_for(Cout, N, a_ph.device, want_stats)
-    taps = tuple((kh // 2, kw // 2, ((kh % 2) * 2 + (kw % 2)) * N) for kh in range(3) for kw in range(3))
-    _tapgemm(a=a_ph, a_term_imgs=4 * N, a_imgs=T * 4 * N, a_bcast=0, n_img=N, H=Ho, W=Wo, a_H=Ho, a_W=Wo,
-             Cc=Cc, a_sw=Cc, a_sh=Wo * Cc, a_sn=Ho * Wo * Cc,
-             b=w, b_term_g=9, b_groups=w.shape[0] * 9, b_batched=0, n_out=Cout, b_sn=Cc, b_sg=Cout * Cc,
-             taps=taps, d=out, d_mode=OUT_F32, d_strides=(Ho * Wo * Cout, Wo * Cout, Cout, 1),
-             bias=bias, bias_mode=BIAS_COL, gn_stats=stats, gn_cpg=cpg)
-    if want_stats:
-        return out, stats
-    return out
+    return tap_conv(a_ph, w, bias, fwd_taps("down", N), n=N, out_hw=(Ho, Wo), want_stats=want_stats)
 
 
 # Split-K GEMMs reduce their k-slices with fp32 atomics (TMA reduce-add), so their results depend on the
@@ -1012,9 +987,9 @@ def tap_conv(a, w, bias, taps, *, n, out_hw, out=None, d_strides=None, planes_ou
     (out_hw) output domain that may differ from a's spatial extent (reads outside a are zero).
     a: planes whose last three dims are (h, w, C) and whose dims between the plane dim and those flatten to the
     image index ([T,N,h,w,C] or the 4-phase [T,4,N,h,w,C]); w: planes [T, slots, Cout, C] (possibly a tap-sliced
-    view); taps: ((dy, dx, img_off), ...).  Serves every conv of the training step that the fixed-shape wrappers
-    above do not: the Discriminator's 4x4 convs (vqgan_arch.py:1160-1197), all data gradients (forward kernel on
-    the transposed weights with negated taps), the parity launches of the strided convs' data gradients."""
+    view); taps: ((dy, dx, img_off), ...).  Serves conv3x3 / conv1x1 / conv3x3_s2 above, the Discriminator's 4x4
+    convs (vqgan_arch.py:1160-1197), all data gradients (forward kernel on the transposed weights with negated taps),
+    the parity launches of the strided convs' data gradients."""
     _need_cuda(a, w)
     T = a.shape[0]
     aH, aW, Cc = a.shape[-3:]
@@ -1086,17 +1061,7 @@ def conv_wgrad(dy, x, taps, dw, *, n, alpha=1.0, k_split=0):
     p.alpha = alpha
     p.nterms = 3 if T == 2 else 1
     p.k_split = k_split
-    _count()
-    if _PROFILE["on"]:
-        e0 = torch.cuda.Event(enable_timing=True)
-        e1 = torch.cuda.Event(enable_timing=True)
-        e0.record()
-        _lib.check(lib.t2h_conv_wgrad(C.byref(p), _stream()))
-        e1.record()
-        algo = 2.0 * N * H * W * Co * Ci * len(taps)
-        _PROFILE["records"].append((algo, algo * p.nterms, e0, e1, ("wgrad", N, H, W, Co, Ci * len(taps))))
-        return dw
-    _lib.check(lib.t2h_conv_wgrad(C.byref(p), _stream()))
+    _launch(lib.t2h_conv_wgrad, p, 2.0 * N * H * W * Co * Ci * len(taps), ("wgrad", N, H, W, Co, Ci * len(taps)))
     return dw
 
 
