@@ -824,7 +824,8 @@ struct TapGemmPlan {
 };
 
 // (tests/test_gpu_tapgemm_paths.py::route restates this selection, tile shape to epilogue mode, and labels its cases
-// with it: a routing change updates it in the same change)
+// with it: a routing change updates it in the same change; tests/test_gpu_tapgemm_rows.py::rows_route does the same
+// for row GEMMs, H == 1 or tile_rows: BN, the MN-major BN >= 64 rule and the epilogue)
 static TapGemmPlan plan_tapgemm(const t2h_tapgemm_params* p) {
   TapGemmPlan L;
   const bool rows_mode = p->H == 1 || p->tile_rows;
@@ -1076,6 +1077,7 @@ extern "C" int t2h_tapgemm(const t2h_tapgemm_params* p, t2h_stream_t stream) {
                   "statistics / gamma / beta, and no other epilogue work");
   }
   // ---- split-K: k-slices of one tile go to different CTAs and are reduce-added into a zeroed output
+  // (tests/test_gpu_tapgemm_rows.py::rows_route restates the k_partials / k_split / accumulate rules below)
   set_k_slices(P, 1);
   if (p->k_partials > 1) {
     T2H_CHECK_ARG(!swap && P.epi_mode == EPI_TMA_F32 && !p->residual && p->bias_mode == T2H_BIAS_NONE &&
