@@ -202,6 +202,13 @@ int t2h_nchw_to_nhwc(const float* x, float* out, int n, int c, int h, int w,
  * (H/2,W/2) x 4 phases for S2D, (H/2,W/2) for MAXPOOL2.  Plane layout: [terms][phases][N][h][w][C]. */
 int t2h_f32_to_planes(const float* x, void* out, int n, int h, int w, int c,
                       int mode, int terms, t2h_stream_t stream);
+/* The operand of every ShapeUNet encoder stage, cat([x, e.view(N,C_e,1,1).expand(N,C_e,H,W)], 1)
+ * (unet_arch.py:657-668), without materialising the broadcast: fp32 NHWC x [N,H,W,C] (any C >= 1; a 1-channel
+ * NCHW tensor is the same bytes) and fp32 e [N,C_e] -> fp16 planes [terms][N][h][w][c_pad] with channels [0,C) from
+ * x, [C,C+C_e) = e[n] and [C+C_e,c_pad) = 0.  mode T2H_CVT_PLAIN (h,w = H,W) or T2H_CVT_MAXPOOL2 (h,w = H/2,W/2;
+ * only x is pooled, the max of a constant window being that constant). */
+int t2h_f32_to_planes_bcast(const float* x, const float* e, void* out, int n, int h, int w, int c, int c_e,
+                            int c_pad, int mode, int terms, t2h_stream_t stream);
 
 /* ------------------------------------------------------------------------
  * GroupNorm(32, C, eps) (+ swish)  — Normalize()/nonlinearity(),
@@ -306,6 +313,17 @@ int t2h_mask_to_ids(const float* mask, int32_t* ids, int b, int hs, int ws, int 
  * head, -1 where head is outside 0..n_heads-1 */
 int t2h_argmax_heads(const float* logits, const int64_t* head, int64_t* out, int64_t rows, int n_heads, int ncls,
                      t2h_stream_t stream);
+
+/* ShapeAttrEmbedding.forward (shape_attr_embedding_arch.py:23-36) in fp32, one CTA per image:
+ * h_i = W2_i . lrelu(W1_i[:, attr[b][i]] + b1_i) + b2_i for the n_attr attributes, then
+ * out[b] = Wf2 . lrelu(Wf1 . cat(h_0..h_{n_attr-1}) + bf1) + bf2 (LeakyReLU slope 0.01).
+ * attr int64 [b][n_attr]; w1t [sum(cls_num)][dim] holds the columns of every W1_i, attribute i's at rows
+ * cls_off[i] .. cls_off[i+1]-1 (cls_off int32 [n_attr+1]); b1, b2 [n_attr][dim]; w2 [n_attr][dim][dim];
+ * wf1 [out_dim][n_attr*dim]; bf1, bf2 [out_dim]; wf2 [out_dim][out_dim]; out fp32 [b][out_dim].  An attribute
+ * outside 0..cls_num-1 (which callers reject before the launch, as F.one_hot does) yields NaN for its image. */
+int t2h_shape_attr_embed(const int64_t* attr, const int32_t* cls_off, const float* w1t, const float* b1,
+                         const float* w2, const float* b2, const float* wf1, const float* bf1, const float* wf2,
+                         const float* bf2, float* out, int b, int n_attr, int dim, int out_dim, t2h_stream_t stream);
 
 /* x[b,t,:] = tok_emb[idx] + pos_emb[t] + segm_emb[segm] + tex_emb[tex]  (:251-266) fp32 */
 int t2h_embed_sum(const int64_t* idx, const int64_t* segm, const int64_t* tex,

@@ -76,6 +76,7 @@ SIGNATURES = {
     "t2h_nhwc_to_nchw": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "t2h_nchw_to_nhwc": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "t2h_f32_to_planes": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "t2h_f32_to_planes_bcast": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "t2h_gn_stats": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "t2h_gn_apply": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _I, _I, _P]),
     "t2h_add_inplace": (_I, [_P, _P, _L, _P]),
@@ -95,6 +96,7 @@ SIGNATURES = {
     "t2h_splitk_reduce_ln": (_I, [_P, _I, _L, _P, _P, _P, _P, _P, _F, _P, _I, _P, _L, _L, _I, _P]),
     "t2h_pack_u8": (_I, [_P, _P, _I, _I, _I, _I, _F, _F, _P]),
     "t2h_argmax_heads": (_I, [_P, _P, _P, _L, _I, _I, _P]),
+    "t2h_shape_attr_embed": (_I, [_P] * 11 + [_I, _I, _I, _I, _P]),
     "t2h_f32_to_planes_t": (_I, [_P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "t2h_planes_transpose": (_I, [_P, _P, _I, _I, _I, _L, _L, _L, _L, _L, _L, _I, _P]),
     "t2h_colsum": (_I, [_P, _P, _L, _I, _P]),

@@ -174,6 +174,61 @@ __global__ void f32_to_planes_kernel(const float* __restrict__ x, __half* __rest
   }
 }
 
+// fp32 NHWC x [N,H,W,C] plus a per-image broadcast block e [N,Ce] -> planes [T,N,oh,ow,c_pad]
+// (t2h_f32_to_planes_bcast).  One thread = 8 output channels of one output position.  8-channel groups that lie
+// inside x with C % 4 == 0 take the vector loads; the rest (C = 1 for the pose input, the x / e / zero boundary)
+// go element by element.
+__global__ void f32_to_planes_bcast_kernel(const float* __restrict__ x, const float* __restrict__ e,
+                                           __half* __restrict__ out, int N, int H, int W, int C, int Ce, int c_pad,
+                                           int pool, int terms, long long plane) {
+  const int c8 = c_pad >> 3;
+  const int oh_n = pool ? H / 2 : H, ow_n = pool ? W / 2 : W;
+  const long long total = (long long)N * oh_n * ow_n * c8;
+  const bool vec = (C & 3) == 0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c0 = (int)(i % c8) * 8;
+    long long r = i / c8;
+    const int ow = (int)(r % ow_n); r /= ow_n;
+    const int oh = (int)(r % oh_n);
+    const int n = (int)(r / oh_n);
+    const int ih = pool ? 2 * oh : oh, iw = pool ? 2 * ow : ow;
+    const float* b = x + (((long long)n * H + ih) * W + iw) * C;
+    const long long dW = C, dH = (long long)W * C;
+    float f[8];
+    if (vec && c0 + 8 <= C) {
+      load8(b + c0, f);
+      if (pool) {
+        float g[8];
+        load8(b + c0 + dW, g);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) f[k] = fmaxf(f[k], g[k]);
+        load8(b + c0 + dH, g);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) f[k] = fmaxf(f[k], g[k]);
+        load8(b + c0 + dH + dW, g);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) f[k] = fmaxf(f[k], g[k]);
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const int c = c0 + k;
+        float v = 0.f;
+        if (c < C) {
+          v = __ldg(b + c);
+          if (pool)
+            v = fmaxf(fmaxf(v, __ldg(b + dW + c)), fmaxf(__ldg(b + dH + c), __ldg(b + dH + dW + c)));
+        } else if (c < C + Ce) {
+          v = __ldg(e + (long long)n * Ce + (c - C));
+        }
+        f[k] = v;
+      }
+    }
+    store_split8(f, out, i * 8, plane, terms);
+  }
+}
+
 // ----------------------------------------------------------------------------
 // GroupNorm statistics: stats[n][g] += (sum, sumsq) in fp64
 // grid (chunks, N); a thread owns one float4 channel slot and walks pixels.
@@ -686,6 +741,53 @@ __global__ void argmax_heads_kernel(const float* __restrict__ logits, const long
   if (lane == 0) out[m] = bi == 0x7fffffff ? 0 : bi;
 }
 
+// ShapeAttrEmbedding (t2h_shape_attr_embed): one CTA per image, the four layers one after another through shared
+// memory; each output element is one thread's fp32 dot product.  The one-hot Linear is a column gather.
+__device__ __forceinline__ float lrelu001(float v) { return v >= 0.f ? v : 0.01f * v; }
+
+__global__ void shape_attr_embed_kernel(const long long* __restrict__ attr, const int* __restrict__ cls_off,
+                                        const float* __restrict__ w1t, const float* __restrict__ b1,
+                                        const float* __restrict__ w2, const float* __restrict__ b2,
+                                        const float* __restrict__ wf1, const float* __restrict__ bf1,
+                                        const float* __restrict__ wf2, const float* __restrict__ bf2,
+                                        float* __restrict__ out, int A, int D, int O) {
+  extern __shared__ float sm[];
+  float* h0 = sm;            // [A*D] lrelu(W1_i[:, a_i] + b1_i)
+  float* h1 = h0 + A * D;    // [A*D] the concatenated per-attribute embeddings
+  float* f = h1 + A * D;     // [O]   lrelu of the first fusion layer
+  const int n = blockIdx.x;
+  const int AD = A * D;
+  for (int t = threadIdx.x; t < AD; t += blockDim.x) {
+    const int i = t / D, j = t - i * D;
+    const long long a = attr[(long long)n * A + i];
+    const int ncls = cls_off[i + 1] - cls_off[i];
+    h0[t] = (a >= 0 && a < ncls) ? lrelu001(w1t[(long long)(cls_off[i] + a) * D + j] + b1[t])
+                                 : __int_as_float(0x7fc00000);
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < AD; t += blockDim.x) {
+    const int i = t / D;
+    const float* w = w2 + (long long)t * D;
+    float s = 0.f;
+    for (int k = 0; k < D; ++k) s = fmaf(w[k], h0[i * D + k], s);
+    h1[t] = s + b2[t];
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < O; t += blockDim.x) {
+    const float* w = wf1 + (long long)t * AD;
+    float s = 0.f;
+    for (int k = 0; k < AD; ++k) s = fmaf(w[k], h1[k], s);
+    f[t] = lrelu001(s + bf1[t]);
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < O; t += blockDim.x) {
+    const float* w = wf2 + (long long)t * O;
+    float s = 0.f;
+    for (int k = 0; k < O; ++k) s = fmaf(w[k], f[k], s);
+    out[(long long)n * O + t] = s + bf2[t];
+  }
+}
+
 }  // namespace t2h
 
 using namespace t2h;
@@ -738,6 +840,23 @@ int t2h_f32_to_planes(const float* x, void* out, int n, int h, int w, int c, int
   const long long work = out_elems / 8;  // (tests/test_gpu_image_kernels.py::f32_to_planes_route restates this grid)
   f32_to_planes_kernel<<<grid_for(work, 256), 256, 0, as_stream(stream)>>>(
       x, reinterpret_cast<__half*>(out), n, h, w, c, mode, terms, out_elems);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_f32_to_planes_bcast(const float* x, const float* e, void* out, int n, int h, int w, int c, int c_e,
+                            int c_pad, int mode, int terms, t2h_stream_t stream) {
+  T2H_CHECK_ARG(x && out && n > 0 && h > 0 && w > 0 && c > 0 && c_e >= 0 && (e || c_e == 0),
+                "f32_to_planes_bcast: bad shape");
+  T2H_CHECK_ARG(c_pad >= c + c_e && c_pad % 8 == 0, "f32_to_planes_bcast: c_pad=%d must be >= %d and a multiple of 8",
+                c_pad, c + c_e);
+  T2H_CHECK_ARG(mode == T2H_CVT_PLAIN || mode == T2H_CVT_MAXPOOL2, "f32_to_planes_bcast: mode=%d", mode);
+  T2H_CHECK_ARG(mode != T2H_CVT_MAXPOOL2 || (h >= 2 && w >= 2), "f32_to_planes_bcast: MAXPOOL2 needs H,W >= 2");
+  T2H_CHECK_ARG(terms == 1 || terms == 2, "f32_to_planes_bcast: terms=%d", terms);
+  const int pool = mode == T2H_CVT_MAXPOOL2;
+  const long long out_elems = (long long)n * (pool ? h / 2 : h) * (pool ? w / 2 : w) * c_pad;
+  f32_to_planes_bcast_kernel<<<grid_for(out_elems / 8, 256), 256, 0, as_stream(stream)>>>(
+      x, e, reinterpret_cast<__half*>(out), n, h, w, c, c_e, c_pad, pool, terms, out_elems);
   T2H_LAUNCH_OK();
   return T2H_OK;
 }
@@ -925,6 +1044,21 @@ int t2h_argmax_heads(const float* logits, const int64_t* head, int64_t* out, int
   const int warps = 8;
   argmax_heads_kernel<<<(unsigned)ceil_div64(rows, warps), warps * 32, 0, as_stream(stream)>>>(
       logits, reinterpret_cast<const long long*>(head), reinterpret_cast<long long*>(out), rows, n_heads, ncls);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_shape_attr_embed(const int64_t* attr, const int32_t* cls_off, const float* w1t, const float* b1,
+                         const float* w2, const float* b2, const float* wf1, const float* bf1, const float* wf2,
+                         const float* bf2, float* out, int b, int n_attr, int dim, int out_dim, t2h_stream_t stream) {
+  T2H_CHECK_ARG(attr && cls_off && w1t && b1 && w2 && b2 && wf1 && bf1 && wf2 && bf2 && out,
+                "shape_attr_embed: null operand");
+  T2H_CHECK_ARG(b > 0 && n_attr > 0 && dim > 0 && out_dim > 0, "shape_attr_embed: bad shape");
+  const size_t smem = (size_t)(2 * n_attr * dim + out_dim) * sizeof(float);
+  T2H_CHECK_ARG(smem <= 48 * 1024, "shape_attr_embed: n_attr*dim=%d, out_dim=%d too large", n_attr * dim, out_dim);
+  shape_attr_embed_kernel<<<b, 128, smem, as_stream(stream)>>>(reinterpret_cast<const long long*>(attr), cls_off,
+                                                               w1t, b1, w2, b2, wf1, bf1, wf2, bf2, out, n_attr,
+                                                               dim, out_dim);
   T2H_LAUNCH_OK();
   return T2H_OK;
 }

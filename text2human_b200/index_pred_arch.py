@@ -97,6 +97,35 @@ class UpConvBlock(nn.Module):
         return self.conv_block.forward_planes(torch.cat((skip, up), dim=-1))     # torch.cat([skip, x], dim=1) :107
 
 
+def build_unet_stages(net, in_channels, base_channels, num_stages, enc_num_convs, dec_num_convs, extra_in=0):
+    """net.encoder / net.decoder with the reference's stage layout (UNet :420-458, ShapeUNet :619-655): stage i is
+    [MaxPool2d(2) for i > 0,] BasicConvBlock(C_in + extra_in -> base * 2**i); ShapeUNet's extra_in is the width of
+    the attribute embedding concatenated to every stage's input"""
+    assert len(enc_num_convs) == num_stages and len(dec_num_convs) == num_stages - 1
+    net.num_stages = num_stages
+    net.encoder = nn.ModuleList()
+    net.decoder = nn.ModuleList()
+    for i in range(num_stages):
+        blk = []
+        if i != 0:
+            blk.append(nn.MaxPool2d(kernel_size=2))
+            net.decoder.append(UpConvBlock(base_channels * 2**i, base_channels * 2**(i - 1),
+                                           base_channels * 2**(i - 1), dec_num_convs[i - 1]))
+        blk.append(BasicConvBlock(in_channels + extra_in, base_channels * 2**i, enc_num_convs[i]))
+        net.encoder.append(nn.Sequential(*blk))
+        in_channels = base_channels * 2**i
+
+
+def unet_decode(decoder, enc):
+    """the UNet decoder (reference :467-471): fp32 NHWC encoder outputs -> dec_outs, coarsest first"""
+    x = enc[-1]
+    dec = [x]
+    for i in reversed(range(len(decoder))):
+        x = decoder[i].forward_planes(enc[i], x)
+        dec.append(x)
+    return dec
+
+
 class UNet(nn.Module):
     """UNet backbone with the reference's defaults (stride-1 stages, MaxPool2d(2) between them, InterpConv
     upsampling).  forward(x NCHW) -> list of num_stages NCHW maps, coarsest first (reference :460-471)."""
@@ -104,19 +133,7 @@ class UNet(nn.Module):
     def __init__(self, in_channels=3, base_channels=64, num_stages=5, enc_num_convs=(2, 2, 2, 2, 2),
                  dec_num_convs=(2, 2, 2, 2)):
         super().__init__()
-        assert len(enc_num_convs) == num_stages and len(dec_num_convs) == num_stages - 1
-        self.num_stages = num_stages
-        self.encoder = nn.ModuleList()
-        self.decoder = nn.ModuleList()
-        for i in range(num_stages):
-            blk = []
-            if i != 0:
-                blk.append(nn.MaxPool2d(kernel_size=2))
-                self.decoder.append(UpConvBlock(base_channels * 2**i, base_channels * 2**(i - 1),
-                                                base_channels * 2**(i - 1), dec_num_convs[i - 1]))
-            blk.append(BasicConvBlock(in_channels, base_channels * 2**i, enc_num_convs[i]))
-            self.encoder.append(nn.Sequential(*blk))
-            in_channels = base_channels * 2**i
+        build_unet_stages(self, in_channels, base_channels, num_stages, enc_num_convs, dec_num_convs)
 
     @torch.no_grad()
     def forward_nhwc(self, x, nhwc_in=False):
@@ -130,11 +147,7 @@ class UNet(nn.Module):
                 a = ops.f32_to_planes(x, ops.CVT_MAXPOOL2)
             x = stage[-1].forward_planes(a)
             enc.append(x)
-        dec = [x]
-        for i in reversed(range(len(self.decoder))):
-            x = self.decoder[i].forward_planes(enc[i], x)
-            dec.append(x)
-        return dec
+        return unet_decode(self.decoder, enc)
 
     def forward(self, x):
         return [ops.nhwc_to_nchw(d) for d in self.forward_nhwc(x)]

@@ -595,6 +595,26 @@ def f32_to_planes(x, mode=CVT_PLAIN, terms=None):
     return out
 
 
+def f32_to_planes_bcast(x, e, mode=CVT_PLAIN, terms=None):
+    """fp32 NHWC x [N,H,W,C] (any C) and fp32 e [N,Ce] -> planes [T,N,h,w,c_pad] of
+    cat([x, e broadcast over h,w], channels), zero-padded to c_pad = C+Ce rounded up to 8.
+    PLAIN: (h,w) = (H,W); MAXPOOL2: (H/2,W/2), the pooled x (a constant channel pools to itself)."""
+    _need_cuda(x, e)
+    assert mode in (CVT_PLAIN, CVT_MAXPOOL2), mode
+    x, e = _f32c(x), _f32c(e)
+    N, H, W, Cc = x.shape
+    Ce = e.shape[1]
+    assert e.shape == (N, Ce), (x.shape, e.shape)
+    terms = terms or get_terms()
+    cp = (Cc + Ce + 7) // 8 * 8
+    hw = (H // 2, W // 2) if mode == CVT_MAXPOOL2 else (H, W)
+    out = torch.empty((terms, N) + hw + (cp,), dtype=torch.float16, device=x.device)
+    _count(1)
+    _lib.check(_lib.load().t2h_f32_to_planes_bcast(_ptr(x), _ptr(e), _ptr(out), N, H, W, Cc, Ce, cp, mode, terms,
+                                                   _stream()))
+    return out
+
+
 def group_norm(x, gamma, beta, *, swish, groups=32, eps=1e-6, terms=None, stats=None):
     """GroupNorm(32, C, eps=1e-6) (+ swish) of fp32 NHWC x -> planes [T,N,H,W,C].
     ``stats``: (sum, sumsq) [N,groups,2] fp64 already accumulated by the producer's epilogue."""
@@ -962,6 +982,23 @@ def argmax_heads(logits, head):
     out = torch.empty((M,), dtype=torch.int64, device=logits.device)
     _count(1)
     _lib.check(_lib.load().t2h_argmax_heads(_ptr(logits), _ptr(head.contiguous()), _ptr(out), M, G, ncls, _stream()))
+    return out
+
+
+def shape_attr_embed(attr, packed):
+    """ShapeAttrEmbedding forward: attr int64 [B,n_attr] (already range-checked) -> fp32 [B,out_dim].
+    packed: dict from ShapeAttrEmbedding's packed-parameter cache (cls_off, w1t, b1, w2, b2, wf1, bf1, wf2, bf2)."""
+    p = packed
+    _need_cuda(attr, p["w1t"])
+    attr = attr.to(torch.int64).contiguous()
+    B, A = attr.shape
+    D, O = p["b1"].shape[1], p["bf1"].shape[0]
+    assert p["cls_off"].numel() == A + 1 and p["b1"].shape[0] == A
+    out = torch.empty((B, O), dtype=torch.float32, device=attr.device)
+    _count(1)
+    _lib.check(_lib.load().t2h_shape_attr_embed(
+        _ptr(attr), _ptr(p["cls_off"]), _ptr(p["w1t"]), _ptr(p["b1"]), _ptr(p["w2"]), _ptr(p["b2"]), _ptr(p["wf1"]),
+        _ptr(p["bf1"]), _ptr(p["wf2"]), _ptr(p["bf2"]), _ptr(out), B, A, D, O, _stream()))
     return out
 
 

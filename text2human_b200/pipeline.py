@@ -8,6 +8,7 @@ points so no layout round trip happens between encoder, quantizer and decoder:
   HierarchyVQSpatialTextureAwareModel.top_encode/bot_encode/decode/forward_step
                                                        models/hierarchy_vqgan_model.py:215-239
   BaseSampleModel.sample_fn                            models/sample_model.py:256-328
+  SampleFromParsingModel / SampleFromPoseModel         models/sample_model.py:215-254, :343-436
 
 Training-only members of the reference wrappers (losses, optimisers, LPIPS,
 discriminator, logging) are outside this round's scope.
@@ -18,6 +19,7 @@ import torch.nn as nn
 
 from . import ops
 from .index_pred_arch import MultiHeadFCNHead, UNet, bot_index_prediction
+from .parsing_gen_arch import FCNHead, ShapeAttrEmbedding, ShapeUNet, generate_parsing_map
 from .transformer_arch import TransformerMultiHead
 from .vqgan_arch import (Decoder, DecoderRes, Encoder, VectorQuantizer, VectorQuantizerSpatialTextureAware,
                          VectorQuantizerTexture, conv1x1_nhwc)
@@ -446,6 +448,61 @@ class SampleFromParsingModel(nn.Module):
         if save_dir is not None and img_name is not None:
             save_images(dec, save_dir, img_name)
         return dec
+
+
+class SampleFromPoseModel(SampleFromParsingModel):
+    """pose + shape attributes + texture attributes -> image: ``SampleFromPoseModel.inference``
+    (sample_model.py:363-436) with the reference's component names and ``opt`` keys (configs/sample_from_pose.yml):
+    parsing generator (ShapeAttrEmbedding -> ShapeUNet -> FCNHead -> argmax) -> texture mask -> everything
+    ``SampleFromParsingModel.sample_and_refine`` runs.  The whole batch goes through every stage at once."""
+
+    def __init__(self, opt):
+        super().__init__(opt)
+        self.shape_attr_embedder = ShapeAttrEmbedding(dim=opt['shape_embedder_dim'],
+                                                      out_dim=opt['shape_embedder_out_dim'],
+                                                      cls_num_list=opt['shape_attr_class_num'])
+        self.shape_parsing_encoder = ShapeUNet(in_channels=opt['shape_encoder_in_channels'],
+                                               attr_embedding=opt['shape_embedder_out_dim'])
+        self.shape_parsing_decoder = FCNHead(
+            in_channels=opt['shape_fc_in_channels'], in_index=opt['shape_fc_in_index'],
+            channels=opt['shape_fc_channels'], num_convs=opt['shape_fc_num_convs'],
+            concat_input=opt['shape_fc_concat_input'], dropout_ratio=opt['shape_fc_dropout_ratio'],
+            num_classes=opt['shape_fc_num_classes'], align_corners=opt['shape_fc_align_corners'])
+
+    def load_shape_generation_models(self, path=None):
+        """parsing_gen.pth: {'embedder', 'encoder', 'decoder'} state dicts, loaded strictly (sample_model.py:397-410)"""
+        ck = torch.load(path or self.opt['pretrained_parsing_gen'], map_location="cpu")
+        for name, key in (("shape_attr_embedder", "embedder"), ("shape_parsing_encoder", "encoder"),
+                          ("shape_parsing_decoder", "decoder")):
+            getattr(self, name).load_state_dict(ck[key], strict=True)
+            getattr(self, name).eval()
+
+    @torch.no_grad()
+    def generate_parsing_map(self, pose, shape_attr):
+        """pose fp32 [B,1,H,W], shape attributes int [B,15] -> float parsing map [B,1,H,W]"""
+        return generate_parsing_map(self.shape_attr_embedder, self.shape_parsing_encoder, self.shape_parsing_decoder,
+                                    pose, shape_attr)
+
+    @torch.no_grad()
+    def generate(self, pose, shape_attr, upper, lower, outer, temp=1.0, sample_steps=None, generator=None,
+                 save_dir=None, img_name=None):
+        """pose [B,1,H,W], shape attributes [B,15], fused texture attributes upper / lower / outer [B] (17 = none)
+        -> images [B,3,H,W] in [0,1] (and the files, with ``save_dir`` / ``img_name``)"""
+        dev = self.shape_attr_embedder.fusion[0].weight.device
+        segm = self.generate_parsing_map(pose.to(dev), shape_attr.to(dev))
+        attrs = torch.stack([torch.as_tensor(a, device=dev).view(-1) for a in (upper, lower, outer)], 1)
+        texture_mask = ops.texture_mask(segm, attrs)
+        return self.sample_and_refine(segm, texture_mask, temp=temp, sample_steps=sample_steps, generator=generator,
+                                      save_dir=save_dir, img_name=img_name)
+
+    @torch.no_grad()
+    def inference(self, data_loader, save_dir, generator=None):
+        """DeepFashionAttrPoseDataset batches ('densepose', 'shape_attr', '*_fused_attr', 'img_name') -> one image
+        file per 'img_name' under save_dir (sample_model.py:425-436)"""
+        for data in data_loader:
+            self.generate(data['densepose'], data['shape_attr'], data['upper_fused_attr'], data['lower_fused_attr'],
+                          data['outer_fused_attr'], sample_steps=self.opt.get('sample_steps'), generator=generator,
+                          save_dir=save_dir, img_name=list(data['img_name']))
 
 
 def save_images(images, save_dir, names):
