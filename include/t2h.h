@@ -218,7 +218,8 @@ int t2h_f32_to_planes_bcast(const float* x, const float* e, void* out, int n, in
  * by the caller (or produced by t2h_tapgemm's gn_stats epilogue instead). */
 int t2h_gn_stats(const float* x, double* stats, int n, int hw, int c, int groups,
                  t2h_stream_t stream);
-/* y = act(gn(x)*gamma+beta) -> fp16 planes NHWC; swish: 0 none, 1 swish (nonlinearity(), :513-517), 2 LeakyReLU(0.2).
+/* y = act(gn(x)*gamma+beta) -> fp16 planes NHWC; swish: 0 none, 1 swish (nonlinearity(), :513-517), 2 LeakyReLU(0.2),
+ * 3 ReLU (mmcv ConvModule of ShapeUNet / FCNHead).
  * With n = 1, hw = N*H*W and groups = c the same two kernels are BatchNorm2d in training mode (batch statistics,
  * eps 1e-5) of the Discriminator (vqgan_arch.py:1178,1193). */
 int t2h_gn_apply(const float* x, const double* stats, const float* gamma,
@@ -430,13 +431,20 @@ int t2h_conv_wgrad(const t2h_conv_wgrad_params* p, t2h_stream_t stream);
  * produced them.  dx = add (optional) + dL/dx as fp32 and / or fp16 planes (either may be NULL, not both: a
  * gradient only the following conv gradients consume needs no fp32 copy); dgamma/dbeta accumulated (each may be
  * NULL, independently of the other).  c % 4 == 0, c <= 2048.  ws: 2*n*c doubles of scratch.  act: 0 none,
- * 1 swish, 2 LeakyReLU(0.2).  dx_colsum (optional, [c], accumulated): column sums of the dx written = the bias gradient of the conv whose output x is.  sums_ready != 0: ws already
+ * 1 swish, 2 LeakyReLU(0.2), 3 ReLU (the gradient passes where t2h_gn_apply's output is positive).  dx_colsum (optional, [c], accumulated): column sums of the dx written = the bias gradient of the conv whose output x is.  sums_ready != 0: ws already
  * holds pass 1's per-(image, channel) sums {sum du, sum du*xhat} -- the data-gradient conv that produced dy
  * accumulated them in its epilogue (t2h_tapgemm_params.nb_sums) -- and only the apply pass runs. */
 int t2h_norm_bwd(const float* x, const double* stats, const float* gamma, const float* beta, const float* dy,
                  const float* add, float* dx, void* dx_planes, int terms, float* dgamma, float* dbeta, double* ws,
                  int n, int hw, int c, int groups, float eps, int act, float* dx_colsum, int sums_ready,
                  t2h_stream_t stream);
+/* t2h_norm_bwd with dy first multiplied by a per-(image, channel) factor dy_scale [n*hw/img_hw][c] (image =
+ * pixel / img_hw over the whole normalisation domain): the Dropout2d between FCNHead's ConvModule and conv_seg
+ * (fcn_arch.py:151-156), whose kept channels are scaled by 1/(1-p), folded into the norm backward's two passes. */
+int t2h_norm_bwd_drop(const float* x, const double* stats, const float* gamma, const float* beta, const float* dy,
+                      const float* dy_scale, int img_hw, float* dx, void* dx_planes, int terms, float* dgamma,
+                      float* dbeta, double* ws, int n, int hw, int c, int groups, float eps, int act,
+                      t2h_stream_t stream);
 /* BatchNorm2d running statistics: r = (1-momentum) r + momentum * batch (unbiased variance); stats [c][2] */
 int t2h_bn_update_running(const double* stats, float* running_mean, float* running_var, int64_t count,
                           float momentum, int c, t2h_stream_t stream);
@@ -489,6 +497,45 @@ int t2h_axpy_dev(const float* a, const float* b, const float* w, float* out, int
 int t2h_sample_step(const float* logits, const float* u, const int64_t* tex, int64_t* x_t, uint8_t* unmasked,
                     int64_t rows, int ncls, int n_heads, float inv_t, float inv_temp, uint64_t seed, uint32_t step,
                     int64_t cont_stride, t2h_stream_t stream);
+
+/* ------------------------------------------------------------------------
+ * Training the parsing generator (ParsingGenModel.optimize_parameters, parsing_gen_model.py:80-95)
+ * ---------------------------------------------------------------------- */
+/* t2h_gn_apply's normalisation (act 0-3) with an fp32 NHWC output `out` and / or fp16 planes `out_planes` (either
+ * may be NULL, not both), and an optional per-(image, channel) factor drop [n*hw/img_hw][c] applied after the
+ * activation: FCNHead's Dropout2d (fcn_arch.py:151-156, factor mask / (1-p)) ahead of the plane split.  c % 8 == 0. */
+int t2h_norm_apply_ex(const float* x, const double* stats, const float* gamma, const float* beta, const float* drop,
+                      int img_hw, float* out, void* out_planes, int n, int hw, int c, int groups, float eps, int act,
+                      int terms, t2h_stream_t stream);
+/* Backward of a ShapeUNet encoder stage's operand [MaxPool2d(2) of] cat([x, e broadcast over H, W]) (unet_arch.py:
+ * 657-668).  da: its gradient fp32 [n][oh][ow][da_ld] as the data-gradient conv wrote it (channels [0,c) x,
+ * [c,c+c_e) e); (oh,ow) = (h/2,w/2) with pool, (h,w) without.  dx (may be NULL) fp32 [n][h][w][c] = (accumulate:
+ * +=) the x part routed to the first maximum of each 2x2 window of the saved pre-pool x [n][h][w][c] (row-major, as
+ * torch), 0 on a dropped odd row / column; any c.  de (may be NULL when c_e == 0) [n][c_e] = (accumulate: +=) the
+ * per-image sums of the e channels, in a fixed order (no atomics); ws: n * 32 * c_e floats of scratch. */
+int t2h_maxpool2_bcast_bwd(const float* da, int da_ld, const float* x, float* dx, int accumulate, float* de,
+                           float* ws, int n, int h, int w, int c, int c_e, int pool, t2h_stream_t stream);
+/* Adjoint of T2H_CVT_BILINEAR2X (InterpConv's nn.Upsample, unet_arch.py:303-304): dy fp32 [n][2h][2w][c] ->
+ * dx [n][h][w][c], each input pixel gathering its output neighbourhood with the forward's weights and border
+ * clamps (deterministic).  c % 4 == 0. */
+int t2h_bilinear2x_bwd(const float* dy, float* dx, int n, int h, int w, int c, t2h_stream_t stream);
+/* Pixel cross-entropy of CrossEntropyLoss (cross_entropy_loss.py:58-80, 187-246: F.cross_entropy(reduction='none',
+ * ignore_index=-100) then .mean()) over fp32 NHWC logits [n][h][w][c] and int64 labels [n][h][w], one pass:
+ * loss_sum[0] += sum over labelled pixels of logsumexp(x) - x[label]; grad_planes (may be NULL) = fp16 planes
+ * [terms][n][h][w][c_pad] of gscale (softmax(x) - onehot(label)), 0 on pad channels and on pixels whose label lies
+ * outside [0,c) (ignore_index; callers reject any other such label before the launch); colsum (may be NULL) [c] +=
+ * column sums of that gradient -- conv_seg's bias gradient.  c_pad % 8 == 0, c <= c_pad <= 256. */
+int t2h_ce_logits(const float* logits, const int64_t* labels, int n, int h, int w, int c, int c_pad, float gscale,
+                  double* loss_sum, void* grad_planes, int terms, float* colsum, t2h_stream_t stream);
+/* ShapeAttrEmbedding backward: the forward of t2h_shape_attr_embed recomputed per image (same operands) and every
+ * parameter's gradient accumulated from d_out fp32 [b][out_dim] into `grad` at element offsets goff int64
+ * [(n_attr+1)*4]: per attribute i (W1_i [dim][cls_i], b1_i [dim], W2_i [dim][dim], b2_i [dim]), then (Wf1
+ * [out_dim][n_attr*dim], bf1, Wf2 [out_dim][out_dim], bf2), the nn.Linear layouts.  fp32, images added in order,
+ * no atomics.  The one-hot Linear's weight gradient is the column attr[b][i] of W1_i. */
+int t2h_shape_attr_embed_bwd(const int64_t* attr, const int32_t* cls_off, const float* w1t, const float* b1,
+                             const float* w2, const float* b2, const float* wf1, const float* bf1, const float* wf2,
+                             const float* bf2, const float* d_out, float* grad, const int64_t* goff, int b,
+                             int n_attr, int dim, int out_dim, t2h_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -123,6 +123,12 @@ SIGNATURES = {
     "t2h_diffaug_bwd": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "t2h_adaptive_weight": (_I, [_P, _P, _L, _F, _F, _F, _P, _P]),
     "t2h_axpy_dev": (_I, [_P, _P, _P, _P, _L, _P]),
+    "t2h_norm_bwd_drop": (_I, [_P, _P, _P, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P]),
+    "t2h_norm_apply_ex": (_I, [_P, _P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _F, _I, _I, _P]),
+    "t2h_maxpool2_bcast_bwd": (_I, [_P, _I, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "t2h_bilinear2x_bwd": (_I, [_P, _P, _I, _I, _I, _I, _P]),
+    "t2h_ce_logits": (_I, [_P, _P, _I, _I, _I, _I, _I, _F, _P, _P, _I, _P, _P]),
+    "t2h_shape_attr_embed_bwd": (_I, [_P] * 13 + [_I, _I, _I, _I, _P]),
     "t2h_sample_step": (_I, [_P, _P, _P, _P, _P, _L, _I, _I, _F, _F, C.c_uint64, C.c_uint32, _L, _P]),
 }
 

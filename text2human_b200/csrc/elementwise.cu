@@ -315,6 +315,7 @@ __global__ void gn_apply_kernel(const float* __restrict__ x, const double* __res
       float y = f[e] * scale[cc * 8 + e] + shift[cc * 8 + e];
       if (swish == 1) y = y / (1.0f + __expf(-y));
       else if (swish == 2) y = y > 0.f ? y : 0.2f * y;  // LeakyReLU(0.2) (Discriminator BatchNorm path)
+      else if (swish == 3) y = y > 0.f ? y : 0.f;        // ReLU (mmcv ConvModule, ShapeUNet / FCNHead)
       f[e] = y;
     }
     store_split8(f, out, ob + i * 8, plane, terms);

@@ -40,14 +40,29 @@ __device__ __forceinline__ void norm_consts(const double* __restrict__ stats, co
   }
 }
 
+// act'(u) of the activation after a norm at element x (xhat its normalised value).  ReLU (act 3) forms u as the
+// apply kernels do (x * scale + shift, scale = gamma * rstd), so the gradient passes exactly where their output
+// is positive (torch's threshold_backward on the output)
+__device__ __forceinline__ float norm_act_grad(float x, float xh, float mean, float rstd, float ga, float be, int act) {
+  if (act == 3) {
+    const float sc = ga * rstd;
+    const float sh = be - mean * sc;
+    return x * sc + sh > 0.f ? 1.0f : 0.0f;
+  }
+  return act_grad(xh * ga + be, act);
+}
+
 // ----------------------------------------------------------------------------
 // GroupNorm / BatchNorm backward, pass 1: S[n][c] = (sum du, sum du*xhat) over the pixels, du = dy * act'(u)
+// (dy first multiplied by dys[image][c] when given: the Dropout2d factor between the activation and its consumer,
+// image = pixel / img_hw over the whole batch)
 // grid (chunks, N); a thread owns 4 consecutive channels and walks pixels (the gn_stats_kernel layout)
 // ----------------------------------------------------------------------------
 __global__ void norm_bwd_reduce_kernel(const float* __restrict__ x, const double* __restrict__ stats,
                                        const float* __restrict__ gamma, const float* __restrict__ beta,
                                        const float* __restrict__ dy, double* __restrict__ S, int HW, int C,
-                                       int groups, float eps, int act, int pix_per_block) {
+                                       int groups, float eps, int act, int pix_per_block,
+                                       const float* __restrict__ dys, int img_hw) {
   extern __shared__ float sm[];  // mean, rstd, gamma, beta [C]; s1, s2 [C]
   float *mean = sm, *rstd = sm + C, *ga = sm + 2 * C, *be = sm + 3 * C, *a1 = sm + 4 * C, *a2 = sm + 5 * C;
   const int n = blockIdx.y;
@@ -67,12 +82,17 @@ __global__ void norm_bwd_reduce_kernel(const float* __restrict__ x, const double
       const float4 xv = __ldg(reinterpret_cast<const float4*>(x + base + (long long)p * C));
       const float4 dv = __ldg(reinterpret_cast<const float4*>(dy + base + (long long)p * C));
       const float xs[4] = {xv.x, xv.y, xv.z, xv.w};
-      const float ds[4] = {dv.x, dv.y, dv.z, dv.w};
+      float ds[4] = {dv.x, dv.y, dv.z, dv.w};
+      if (dys) {
+        const float* f = dys + (((long long)n * HW + p) / img_hw) * C + cs * 4;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) ds[e] *= f[e];
+      }
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int c = cs * 4 + e;
         const float xh = (xs[e] - mean[c]) * rstd[c];
-        const float du = ds[e] * act_grad(xh * ga[c] + be[c], act);
+        const float du = ds[e] * norm_act_grad(xs[e], xh, mean[c], rstd[c], ga[c], be[c], act);
         s1[e] += du;
         s2[e] += du * xh;
       }
@@ -97,7 +117,7 @@ __global__ void norm_bwd_apply_kernel(const float* __restrict__ x, const double*
                                       const float* __restrict__ add, float* __restrict__ dx,
                                       __half* __restrict__ planes, int terms, long long plane, int HW, int C,
                                       int groups, float eps, int act, int pix_per_block,
-                                      float* __restrict__ dx_colsum) {
+                                      float* __restrict__ dx_colsum, const float* __restrict__ dys, int img_hw) {
   extern __shared__ float sm[];  // mean, rstd, gamma, beta, m1, m2, colsum [C]
   float *mean = sm, *rstd = sm + C, *ga = sm + 2 * C, *be = sm + 3 * C, *m1 = sm + 4 * C, *m2 = sm + 5 * C;
   float* csum = sm + 6 * C;
@@ -136,14 +156,19 @@ __global__ void norm_bwd_apply_kernel(const float* __restrict__ x, const double*
     float4 av = make_float4(0.f, 0.f, 0.f, 0.f);
     if (add) av = __ldg(reinterpret_cast<const float4*>(add + o));
     const float xs[4] = {xv.x, xv.y, xv.z, xv.w};
-    const float ds[4] = {dv.x, dv.y, dv.z, dv.w};
+    float ds[4] = {dv.x, dv.y, dv.z, dv.w};
     const float as[4] = {av.x, av.y, av.z, av.w};
+    if (dys) {
+      const float* f = dys + (((long long)n * HW + p_begin + i / c4) / img_hw) * C + c0;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) ds[e] *= f[e];
+    }
     float r[4];
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const int c = c0 + e;
       const float xh = (xs[e] - mean[c]) * rstd[c];
-      const float du = ds[e] * act_grad(xh * ga[c] + be[c], act);
+      const float du = ds[e] * norm_act_grad(xs[e], xh, mean[c], rstd[c], ga[c], be[c], act);
       r[e] = rstd[c] * (du * ga[c] - m1[c] - xh * m2[c]) + as[e];
     }
     if (dx) *reinterpret_cast<float4*>(dx + o) = make_float4(r[0], r[1], r[2], r[3]);  // null: only the planes are consumed
@@ -577,6 +602,8 @@ __global__ void sample_step_kernel(const float* __restrict__ logits, const float
 // (apply), 56 KB at the largest C.  Above the default 48 KB a kernel must be opted in, once per device (the
 // attribute lives in the device's copy of the function); model shapes stay below it and never call this.
 constexpr int kNormBwdMaxC = 2048;
+// chunks per image of the broadcast-channel gradient sums of t2h_maxpool2_bcast_bwd (its ws: n * kBcastChunks * c_e)
+constexpr int kBcastChunks = 32;
 static int smem_opt_in(const void* kernel, size_t bytes, int max_bytes, bool (&configured)[64]) {
   if (bytes <= 48 * 1024) return T2H_OK;
   int dev = 0;
@@ -588,21 +615,16 @@ static int smem_opt_in(const void* kernel, size_t bytes, int max_bytes, bool (&c
   return T2H_OK;
 }
 
-}  // namespace t2h
-
-using namespace t2h;
-
-extern "C" {
-
-int t2h_norm_bwd(const float* x, const double* stats, const float* gamma, const float* beta, const float* dy,
-                 const float* add, float* dx, void* dx_planes, int terms, float* dgamma, float* dbeta, double* ws,
-                 int n, int hw, int c, int groups, float eps, int act, float* dx_colsum, int sums_ready,
-                 t2h_stream_t stream) {
+static int norm_bwd_impl(const float* x, const double* stats, const float* gamma, const float* beta, const float* dy,
+                         const float* add, float* dx, void* dx_planes, int terms, float* dgamma, float* dbeta, double* ws,
+                         int n, int hw, int c, int groups, float eps, int act, float* dx_colsum, int sums_ready,
+                         const float* dy_scale, int img_hw, t2h_stream_t stream) {
   T2H_CHECK_ARG(x && stats && gamma && beta && dy && (dx || dx_planes) && ws && n > 0 && hw > 0, "norm_bwd: bad args");
   T2H_CHECK_ARG(c % groups == 0 && c % 4 == 0 && c <= kNormBwdMaxC, "norm_bwd: C=%d groups=%d unsupported", c,
                 groups);
-  T2H_CHECK_ARG(act >= 0 && act <= 2 && (terms == 1 || terms == 2 || !dx_planes), "norm_bwd: act=%d terms=%d", act,
+  T2H_CHECK_ARG(act >= 0 && act <= 3 && (terms == 1 || terms == 2 || !dx_planes), "norm_bwd: act=%d terms=%d", act,
                 terms);
+  T2H_CHECK_ARG(!dy_scale || (img_hw > 0 && ((long long)n * hw) % img_hw == 0), "norm_bwd: img_hw=%d", img_hw);
   cudaStream_t st = as_stream(stream);
   // (tests/test_gpu_backward_paths.py::norm_bwd_route restates the block, lane and pixels-per-block choices below)
   if (!sums_ready) {  // pass 1 (skipped when the conv that produced dy accumulated the sums in its epilogue)
@@ -623,7 +645,7 @@ int t2h_norm_bwd(const float* x, const double* stats, const float* gamma, const 
                          reduce_configured);
     if (rc) return rc;
     norm_bwd_reduce_kernel<<<dim3(blocks_x, n), block, smem, st>>>(x, stats, gamma, beta, dy, ws, hw, c, groups, eps,
-                                                                   act, ppb);
+                                                                   act, ppb, dy_scale, img_hw);
     T2H_LAUNCH_OK();
   }
   int bx2 = ceil_div(num_sms() * 8, n);
@@ -637,7 +659,7 @@ int t2h_norm_bwd(const float* x, const double* stats, const float* gamma, const 
   if (rc) return rc;
   norm_bwd_apply_kernel<<<dim3(bx2, n), 256, smem2, st>>>(
       x, stats, gamma, beta, dy, ws, add, dx, reinterpret_cast<__half*>(dx_planes), terms, (long long)n * hw * c, hw,
-      c, groups, eps, act, ppb2, dx_colsum);
+      c, groups, eps, act, ppb2, dx_colsum, dy_scale, img_hw);
   T2H_LAUNCH_OK();
   if (dgamma || dbeta) {  // either may be given alone
     norm_bwd_params_kernel<<<ceil_div(c, 128), 128, 0, st>>>(ws, dgamma, dbeta, n, c);
@@ -645,6 +667,366 @@ int t2h_norm_bwd(const float* x, const double* stats, const float* gamma, const 
   }
   return T2H_OK;
 }
+
+// ----------------------------------------------------------------------------
+// Training of the parsing generator (ParsingGenModel.optimize_parameters, parsing_gen_model.py:80-95): the
+// backward of the pieces only the ShapeUNet / FCNHead path has.
+// ----------------------------------------------------------------------------
+// BatchNorm / GroupNorm apply with an fp32 output and / or fp16 planes, and an optional per-(image, channel) factor
+// after the activation (Dropout2d of the FCN head: mask / (1 - p); image = pixel / img_hw over the whole batch).
+// y = act(x * scale + shift) * drop, the gn_apply_kernel arithmetic; grid (chunks, n)
+__global__ void norm_apply_ex_kernel(const float* __restrict__ x, const double* __restrict__ stats,
+                                     const float* __restrict__ gamma, const float* __restrict__ beta,
+                                     const float* __restrict__ drop, int img_hw, float* __restrict__ out,
+                                     __half* __restrict__ planes, int HW, int C, int groups, float eps, int act,
+                                     int terms, long long plane, int pix_per_block) {
+  extern __shared__ float sm[];  // scale[C], shift[C]
+  float* scale = sm;
+  float* shift = sm + C;
+  const int n = blockIdx.y;
+  const int cpg = C / groups;
+  const double cnt = (double)HW * cpg;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const int g = c / cpg;
+    const double s = stats[((long long)n * groups + g) * 2 + 0];
+    const double q = stats[((long long)n * groups + g) * 2 + 1];
+    const double mean = s / cnt;
+    double var = q / cnt - mean * mean;
+    if (var < 0) var = 0;
+    const float rstd = (float)(1.0 / sqrt(var + (double)eps));
+    const float ga = gamma[c] * rstd;
+    scale[c] = ga;
+    shift[c] = beta[c] - (float)mean * ga;
+  }
+  __syncthreads();
+  const int c8 = C >> 3;
+  const long long p_begin = (long long)blockIdx.x * pix_per_block;
+  const long long work = (long long)min((long long)pix_per_block, HW - p_begin) * c8;
+  const long long ob = ((long long)n * HW + p_begin) * C;
+  for (long long i = threadIdx.x; i < work; i += blockDim.x) {
+    const int cc = (int)(i % c8);
+    const long long o = ob + i * 8;
+    const float4 a = __ldg(reinterpret_cast<const float4*>(x + o));
+    const float4 b = __ldg(reinterpret_cast<const float4*>(x + o) + 1);
+    float f[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    const float* dr = drop ? drop + (((long long)n * HW + p_begin + i / c8) / img_hw) * C + cc * 8 : nullptr;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      float y = f[e] * scale[cc * 8 + e] + shift[cc * 8 + e];
+      if (act == 1) y = y / (1.0f + __expf(-y));
+      else if (act == 2) y = y > 0.f ? y : 0.2f * y;
+      else if (act == 3) y = y > 0.f ? y : 0.f;
+      if (dr) y *= dr[e];
+      f[e] = y;
+    }
+    if (out) {
+      reinterpret_cast<float4*>(out + o)[0] = make_float4(f[0], f[1], f[2], f[3]);
+      reinterpret_cast<float4*>(out + o)[1] = make_float4(f[4], f[5], f[6], f[7]);
+    }
+    if (planes) {
+      H8 hi, lo;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) split_f16(f[e], hi.v[e], lo.v[e]);
+      *reinterpret_cast<H8*>(planes + o) = hi;
+      if (terms == 2) *reinterpret_cast<H8*>(planes + plane + o) = lo;
+    }
+  }
+}
+
+// Backward of a ShapeUNet encoder stage's input, [MaxPool2d(2) of] cat([x, e broadcast over H, W]), for the x part:
+// dx[n,ih,iw,c] (+)= da[n,ih/2,iw/2,c] at the first maximum (row-major, as torch's max_pool2d) of its 2x2 window,
+// 0 elsewhere and on a dropped odd row / column; without pooling dx = da's x channels.  One thread per element of
+// dx, so any C; a gather, so no atomics.
+__global__ void maxpool2_bcast_dx_kernel(const float* __restrict__ da, int da_ld, const float* __restrict__ x,
+                                         float* __restrict__ dx, int accumulate, int H, int W, int C, int pool,
+                                         long long total) {
+  const int oh_n = pool ? H / 2 : H, ow_n = pool ? W / 2 : W;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    long long r = i / C;
+    const int iw = (int)(r % W); r /= W;
+    const int ih = (int)(r % H);
+    const int n = (int)(r / H);
+    float g = 0.f;
+    if (!pool) {
+      g = da[(((long long)n * oh_n + ih) * ow_n + iw) * da_ld + c];
+    } else {
+      const int oh = ih >> 1, ow = iw >> 1;
+      if (oh < oh_n && ow < ow_n) {
+        const float* b = x + (((long long)n * H + 2 * oh) * W + 2 * ow) * C + c;
+        const float v[4] = {b[0], b[C], b[(long long)W * C], b[(long long)W * C + C]};
+        float best = v[0];
+        int k = 0;
+#pragma unroll
+        for (int j = 1; j < 4; ++j)
+          if (v[j] > best || isnan(v[j])) { best = v[j]; k = j; }
+        if (k == (ih & 1) * 2 + (iw & 1)) g = da[(((long long)n * oh_n + oh) * ow_n + ow) * da_ld + c];
+      }
+    }
+    dx[i] = accumulate ? dx[i] + g : g;
+  }
+}
+
+// ... and for the broadcast part: partial per-image sums of da's channels [C, C+Ce) over a chunk of pixels, fixed
+// order (a thread walks its pixels, the block's lanes are added in lane order) -> ws[n][chunk][Ce]
+__global__ void bcast_sum_partial_kernel(const float* __restrict__ da, int da_ld, int C, int Ce, int hw,
+                                         int pix_per_chunk, float* __restrict__ ws) {
+  extern __shared__ float part[];  // [lanes][Ce]
+  const int n = blockIdx.y, chunk = blockIdx.x;
+  const int lanes = blockDim.x >= Ce ? blockDim.x / Ce : 1;
+  const int lane = threadIdx.x / (blockDim.x >= Ce ? Ce : blockDim.x);
+  const int p0 = chunk * pix_per_chunk, p1 = min(hw, p0 + pix_per_chunk);
+  if (lane < lanes) {
+    for (int j = threadIdx.x % (blockDim.x >= Ce ? Ce : blockDim.x); j < Ce; j += blockDim.x) {
+      float s = 0.f;
+      for (int p = p0 + lane; p < p1; p += lanes) s += da[((long long)n * hw + p) * da_ld + C + j];
+      part[lane * Ce + j] = s;
+    }
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < Ce; j += blockDim.x) {
+    float s = 0.f;
+    for (int l = 0; l < lanes; ++l) s += part[l * Ce + j];
+    ws[((long long)n * gridDim.x + chunk) * Ce + j] = s;
+  }
+}
+
+__global__ void bcast_sum_final_kernel(const float* __restrict__ ws, int chunks, int n_img, int Ce,
+                                       float* __restrict__ de, int accumulate) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_img * Ce) return;
+  const int n = i / Ce, j = i % Ce;
+  float s = 0.f;
+  for (int k = 0; k < chunks; ++k) s += ws[((long long)n * chunks + k) * Ce + j];
+  de[i] = accumulate ? de[i] + s : s;
+}
+
+// Adjoint of T2H_CVT_BILINEAR2X (nn.Upsample(x2, bilinear, align_corners=False)) as a gather: input row r receives
+// from output rows 2r-1 .. 2r+2 the weights the forward gave it (same source-coordinate arithmetic, border clamps
+// included), likewise for columns.  dy [n][2h][2w][c] -> dx [n][h][w][c], c % 4 == 0; fixed summation order.
+__device__ __forceinline__ float bilinear_w(int o, int r, int n_in) {
+  const float s = fmaxf(0.5f * (o + 0.5f) - 0.5f, 0.f);
+  const int i0 = (int)s, i1 = min(i0 + 1, n_in - 1);
+  const float l = s - i0;
+  return (i0 == r ? 1.f - l : 0.f) + (i1 == r ? l : 0.f);
+}
+
+__global__ void bilinear2x_bwd_kernel(const float* __restrict__ dy, float* __restrict__ dx, int H, int W, int C,
+                                      long long total) {
+  const int c4 = C >> 2;
+  const int H2 = 2 * H, W2 = 2 * W;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int cc = (int)(i % c4);
+    long long r = i / c4;
+    const int s = (int)(r % W); r /= W;
+    const int h = (int)(r % H);
+    const int n = (int)(r / H);
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int oh = max(2 * h - 1, 0); oh <= min(2 * h + 2, H2 - 1); ++oh) {
+      const float wh = bilinear_w(oh, h, H);
+      if (wh == 0.f) continue;
+      for (int ow = max(2 * s - 1, 0); ow <= min(2 * s + 2, W2 - 1); ++ow) {
+        const float ww = bilinear_w(ow, s, W);
+        if (ww == 0.f) continue;
+        const float wgt = wh * ww;
+        const float4 v = __ldg(reinterpret_cast<const float4*>(dy + (((long long)n * H2 + oh) * W2 + ow) * C) + cc);
+        acc.x = fmaf(wgt, v.x, acc.x);
+        acc.y = fmaf(wgt, v.y, acc.y);
+        acc.z = fmaf(wgt, v.z, acc.z);
+        acc.w = fmaf(wgt, v.w, acc.w);
+      }
+    }
+    reinterpret_cast<float4*>(dx)[i] = acc;
+  }
+}
+
+// Pixel cross-entropy (F.cross_entropy(reduction='none', ignore_index) of CrossEntropyLoss, cross_entropy_loss.py)
+// over fp32 NHWC logits [pix][c] and int64 labels [pix], one pass: loss[0] += sum over labelled pixels of
+// logsumexp(x) - x[label]; planes = fp16 [terms][pix][c_pad] of gscale (softmax(x) - onehot), 0 on ignored pixels
+// and pad channels; colsum[c] += column sums of that gradient (conv_seg's bias gradient).  A label outside [0, c)
+// contributes nothing (the caller rejects those that are not ignore_index before the launch).
+// g = c_pad/8 rounded up to a power of two threads share a pixel (8 channels each) and reduce the row's max and
+// sum with shuffles inside their group; blockDim is a multiple of g, so a thread always meets the same channels.
+__global__ void ce_logits_kernel(const float* __restrict__ x, const long long* __restrict__ labels, long long npix,
+                                 int C, int c_pad, int g, float gscale, double* __restrict__ loss,
+                                 __half* __restrict__ planes, int terms, float* __restrict__ colsum) {
+  extern __shared__ double cs_sm[];  // [c_pad]
+  const int sub = threadIdx.x % g, lane = threadIdx.x / g, lanes = blockDim.x / g;
+  const int c0 = sub * 8;
+  const unsigned gmask = g == 32 ? 0xffffffffu : (((1u << g) - 1u) << ((threadIdx.x & 31) & ~(g - 1)));
+  const long long plane = npix * c_pad;
+  for (int c = threadIdx.x; c < c_pad; c += blockDim.x) cs_sm[c] = 0.0;
+  __syncthreads();
+  float cs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  double acc = 0.0;
+  for (long long p = (long long)blockIdx.x * lanes + lane; p < npix; p += (long long)gridDim.x * lanes) {
+    const long long lab = __ldg(labels + p);
+    const bool valid = lab >= 0 && lab < C;
+    float v[8];
+    float m = -INFINITY;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int c = c0 + e;
+      v[e] = c < C ? __ldg(x + p * C + c) : -INFINITY;
+      m = fmaxf(m, v[e]);
+    }
+    for (int o = g >> 1; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(gmask, m, o));
+    float s = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) s += c0 + e < C ? expf(v[e] - m) : 0.f;
+    for (int o = g >> 1; o > 0; o >>= 1) s += __shfl_xor_sync(gmask, s, o);
+    if (c0 >= c_pad) continue;  // threads of the group past the padded row (g > c_pad / 8) only help reduce
+    H8 hi, lo;
+    float part = 0.f;
+    const float inv = 1.f / s;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int c = c0 + e;
+      float gr = 0.f;
+      if (valid && c < C) {
+        const bool t = c == (int)lab;
+        gr = gscale * (expf(v[e] - m) * inv - (t ? 1.f : 0.f));
+        if (t) part -= v[e];
+        cs[e] += gr;
+      }
+      split_f16(gr, hi.v[e], lo.v[e]);
+    }
+    if (valid && sub == 0) part += m + logf(s);
+    acc += (double)part;
+    if (planes) {
+      *reinterpret_cast<H8*>(planes + p * c_pad + c0) = hi;
+      if (terms == 2) *reinterpret_cast<H8*>(planes + plane + p * c_pad + c0) = lo;
+    }
+  }
+  block_add(acc, loss);
+  if (colsum) {
+    if (c0 < c_pad) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) atomicAdd(&cs_sm[c0 + e], (double)cs[e]);
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < C; c += blockDim.x) atomicAdd(&colsum[c], (float)cs_sm[c]);
+  }
+}
+
+// ShapeAttrEmbedding backward (shape_attr_embedding_arch.py:23-36; LeakyReLU slope 0.01): one CTA walks the images
+// in order, recomputes each image's forward exactly as shape_attr_embed_kernel does (pre-activations kept) and
+// accumulates every parameter's gradient from d_out[b] into `grad` at the element offsets goff: per attribute i
+// (W1_i [dim][cls_i], b1_i, W2_i [dim][dim], b2_i), then (Wf1 [out][n_attr*dim], bf1, Wf2 [out][out], bf2) -- the
+// nn.Linear layouts.  A thread owns fixed gradient elements, images are added in order: deterministic, no atomics.
+// The one-hot Linear's weight gradient is the column a_i of W1_i.
+__global__ void shape_attr_embed_bwd_kernel(const long long* __restrict__ attr, const int* __restrict__ cls_off,
+                                            const float* __restrict__ w1t, const float* __restrict__ b1,
+                                            const float* __restrict__ w2, const float* __restrict__ b2,
+                                            const float* __restrict__ wf1, const float* __restrict__ bf1,
+                                            const float* __restrict__ wf2, const float* __restrict__ bf2,
+                                            const float* __restrict__ d_out, float* __restrict__ grad,
+                                            const long long* __restrict__ goff, int B, int A, int D, int O) {
+  extern __shared__ float sm[];
+  const int AD = A * D;
+  float* p0 = sm;            // [AD] pre-activation of the per-attribute first layers
+  float* h1 = p0 + AD;       // [AD] concatenated per-attribute embeddings
+  float* pf = h1 + AD;       // [O]  pre-activation of the first fusion layer
+  float* d = pf + O;         // [O]  d_out[b]
+  float* dpf = d + O;        // [O]  d pf
+  float* dh1 = dpf + O;      // [AD] d h1
+  float* dp0 = dh1 + AD;     // [AD] d p0
+  auto lr = [](float v) { return v >= 0.f ? v : 0.01f * v; };
+  auto lrg = [](float v) { return v > 0.f ? 1.f : 0.01f; };
+  const long long* gf = goff + 4 * A;
+  for (int b = 0; b < B; ++b) {
+    for (int t = threadIdx.x; t < AD; t += blockDim.x) {
+      const int i = t / D, j = t - i * D;
+      const long long a = attr[(long long)b * A + i];
+      const int ncls = cls_off[i + 1] - cls_off[i];
+      p0[t] = (a >= 0 && a < ncls) ? w1t[(long long)(cls_off[i] + a) * D + j] + b1[t] : 0.f;
+    }
+    for (int t = threadIdx.x; t < O; t += blockDim.x) d[t] = d_out[(long long)b * O + t];
+    __syncthreads();
+    for (int t = threadIdx.x; t < AD; t += blockDim.x) {
+      const int i = t / D;
+      const float* w = w2 + (long long)t * D;
+      float s = 0.f;
+      for (int k = 0; k < D; ++k) s = fmaf(w[k], lr(p0[i * D + k]), s);
+      h1[t] = s + b2[t];
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < O; t += blockDim.x) {
+      const float* w = wf1 + (long long)t * AD;
+      float s = 0.f;
+      for (int k = 0; k < AD; ++k) s = fmaf(w[k], h1[k], s);
+      pf[t] = s + bf1[t];
+    }
+    __syncthreads();
+    // fusion[2]: dWf2 += d f^T, dbf2 += d; d f = Wf2^T d
+    for (int t = threadIdx.x; t < O * O; t += blockDim.x) grad[gf[2] + t] += d[t / O] * lr(pf[t % O]);
+    for (int t = threadIdx.x; t < O; t += blockDim.x) {
+      grad[gf[3] + t] += d[t];
+      float s = 0.f;
+      for (int k = 0; k < O; ++k) s = fmaf(wf2[(long long)k * O + t], d[k], s);
+      dpf[t] = s * lrg(pf[t]);
+    }
+    __syncthreads();
+    // fusion[0]: dWf1 += dpf h1^T, dbf1 += dpf; d h1 = Wf1^T dpf
+    for (int t = threadIdx.x; t < O * AD; t += blockDim.x) grad[gf[0] + t] += dpf[t / AD] * h1[t % AD];
+    for (int t = threadIdx.x; t < O; t += blockDim.x) grad[gf[1] + t] += dpf[t];
+    for (int t = threadIdx.x; t < AD; t += blockDim.x) {
+      float s = 0.f;
+      for (int k = 0; k < O; ++k) s = fmaf(wf1[(long long)k * AD + t], dpf[k], s);
+      dh1[t] = s;
+    }
+    __syncthreads();
+    // attr_i[2]: dW2_i += dh1_i lrelu(p0_i)^T, db2_i += dh1_i
+    for (int t = threadIdx.x; t < AD * D; t += blockDim.x) {
+      const int i = t / (D * D), jk = t - i * D * D, j = jk / D, k = jk - j * D;
+      grad[goff[4 * i + 2] + jk] += dh1[i * D + j] * lr(p0[i * D + k]);
+    }
+    for (int t = threadIdx.x; t < AD; t += blockDim.x) grad[goff[4 * (t / D) + 3] + t % D] += dh1[t];
+    __syncthreads();
+    // d p0_i = (W2_i^T dh1_i) * lrelu'(p0_i); attr_i[0]: column a_i of dW1_i and db1_i
+    for (int t = threadIdx.x; t < AD; t += blockDim.x) {
+      const int i = t / D, k = t - i * D;
+      float s = 0.f;
+      for (int j = 0; j < D; ++j) s = fmaf(w2[((long long)i * D + j) * D + k], dh1[i * D + j], s);
+      dp0[t] = s * lrg(p0[t]);
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < AD; t += blockDim.x) {
+      const int i = t / D, j = t - i * D;
+      const long long a = attr[(long long)b * A + i];
+      const int ncls = cls_off[i + 1] - cls_off[i];
+      if (a >= 0 && a < ncls) grad[goff[4 * i] + (long long)j * ncls + a] += dp0[t];
+      grad[goff[4 * i + 1] + j] += dp0[t];
+    }
+    __syncthreads();
+  }
+}
+
+}  // namespace t2h
+
+using namespace t2h;
+
+extern "C" {
+
+int t2h_norm_bwd(const float* x, const double* stats, const float* gamma, const float* beta, const float* dy,
+                 const float* add, float* dx, void* dx_planes, int terms, float* dgamma, float* dbeta, double* ws,
+                 int n, int hw, int c, int groups, float eps, int act, float* dx_colsum, int sums_ready,
+                 t2h_stream_t stream) {
+  return norm_bwd_impl(x, stats, gamma, beta, dy, add, dx, dx_planes, terms, dgamma, dbeta, ws, n, hw, c, groups, eps,
+                       act, dx_colsum, sums_ready, nullptr, 1, stream);
+}
+
+int t2h_norm_bwd_drop(const float* x, const double* stats, const float* gamma, const float* beta, const float* dy,
+                      const float* dy_scale, int img_hw, float* dx, void* dx_planes, int terms, float* dgamma,
+                      float* dbeta, double* ws, int n, int hw, int c, int groups, float eps, int act,
+                      t2h_stream_t stream) {
+  T2H_CHECK_ARG(dy_scale, "norm_bwd_drop: dy_scale is required");
+  return norm_bwd_impl(x, stats, gamma, beta, dy, nullptr, dx, dx_planes, terms, dgamma, dbeta, ws, n, hw, c, groups,
+                       eps, act, nullptr, 0, dy_scale, img_hw, stream);
+}
+
 
 int t2h_bn_update_running(const double* stats, float* running_mean, float* running_var, int64_t count,
                           float momentum, int c, t2h_stream_t stream) {
@@ -775,6 +1157,97 @@ int t2h_sample_step(const float* logits, const float* u, const int64_t* tex, int
   sample_step_kernel<<<(unsigned)ceil_div64(rows, warps), warps * 32, 0, as_stream(stream)>>>(
       logits, u, reinterpret_cast<const long long*>(tex), reinterpret_cast<long long*>(x_t), unmasked, rows, ncls,
       n_heads, inv_t, inv_temp, (unsigned long long)seed, step, cont_stride);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+// ---- parsing-generator training (ParsingGenModel.optimize_parameters, parsing_gen_model.py:80-95)
+int t2h_norm_apply_ex(const float* x, const double* stats, const float* gamma, const float* beta, const float* drop,
+                      int img_hw, float* out, void* out_planes, int n, int hw, int c, int groups, float eps, int act,
+                      int terms, t2h_stream_t stream) {
+  T2H_CHECK_ARG(x && stats && gamma && beta && (out || out_planes) && n > 0 && hw > 0, "norm_apply_ex: bad args");
+  T2H_CHECK_ARG(c % groups == 0 && c % 8 == 0 && c <= 4096, "norm_apply_ex: C=%d groups=%d unsupported", c, groups);
+  T2H_CHECK_ARG(act >= 0 && act <= 3 && (!out_planes || terms == 1 || terms == 2), "norm_apply_ex: act=%d terms=%d",
+                act, terms);
+  T2H_CHECK_ARG(!drop || (img_hw > 0 && ((long long)n * hw) % img_hw == 0), "norm_apply_ex: img_hw=%d", img_hw);
+  int blocks_x = ceil_div(num_sms() * 8, n);
+  int ppb = ceil_div(hw, blocks_x);
+  if (ppb < 16) ppb = 16;
+  blocks_x = ceil_div(hw, ppb);
+  norm_apply_ex_kernel<<<dim3(blocks_x, n), 256, 2 * c * sizeof(float), as_stream(stream)>>>(
+      x, stats, gamma, beta, drop, img_hw, out, reinterpret_cast<__half*>(out_planes), hw, c, groups, eps, act, terms,
+      (long long)n * hw * c, ppb);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_maxpool2_bcast_bwd(const float* da, int da_ld, const float* x, float* dx, int accumulate, float* de,
+                           float* ws, int n, int h, int w, int c, int c_e, int pool, t2h_stream_t stream) {
+  T2H_CHECK_ARG(da && n > 0 && h > 0 && w > 0 && c >= 0 && c_e >= 0 && da_ld >= c + c_e,
+                "maxpool2_bcast_bwd: bad args");
+  T2H_CHECK_ARG(!dx || (c > 0 && (x || !pool)), "maxpool2_bcast_bwd: dx needs c > 0 and, pooled, the saved x");
+  T2H_CHECK_ARG(!c_e || (de && ws), "maxpool2_bcast_bwd: d_e needs de and ws");
+  T2H_CHECK_ARG(!pool || (h >= 2 && w >= 2), "maxpool2_bcast_bwd: pooling needs H, W >= 2");
+  cudaStream_t st = as_stream(stream);
+  if (dx) {
+    const long long total = (long long)n * h * w * c;
+    maxpool2_bcast_dx_kernel<<<grid_cap(total, 256), 256, 0, st>>>(da, da_ld, x, dx, accumulate, h, w, c, pool,
+                                                                    total);
+    T2H_LAUNCH_OK();
+  }
+  if (c_e) {
+    const int hw = (pool ? h / 2 : h) * (pool ? w / 2 : w);
+    const int chunks = min(kBcastChunks, ceil_div(hw, 64));
+    const int ppc = ceil_div(hw, chunks);
+    const int block = 256;
+    const int lanes = block >= c_e ? block / c_e : 1;
+    const size_t smem = (size_t)lanes * c_e * sizeof(float);
+    T2H_CHECK_ARG(smem <= 48 * 1024, "maxpool2_bcast_bwd: c_e=%d too large", c_e);
+    bcast_sum_partial_kernel<<<dim3(chunks, n), block, smem, st>>>(da, da_ld, c, c_e, hw, ppc, ws);
+    T2H_LAUNCH_OK();
+    bcast_sum_final_kernel<<<ceil_div(n * c_e, 128), 128, 0, st>>>(ws, chunks, n, c_e, de, accumulate);
+    T2H_LAUNCH_OK();
+  }
+  return T2H_OK;
+}
+
+int t2h_bilinear2x_bwd(const float* dy, float* dx, int n, int h, int w, int c, t2h_stream_t stream) {
+  T2H_CHECK_ARG(dy && dx && n > 0 && h > 0 && w > 0 && c > 0 && c % 4 == 0, "bilinear2x_bwd: bad args");
+  const long long total = (long long)n * h * w * (c / 4);
+  bilinear2x_bwd_kernel<<<grid_cap(total, 256), 256, 0, as_stream(stream)>>>(dy, dx, h, w, c, total);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_ce_logits(const float* logits, const int64_t* labels, int n, int h, int w, int c, int c_pad, float gscale,
+                  double* loss_sum, void* grad_planes, int terms, float* colsum, t2h_stream_t stream) {
+  T2H_CHECK_ARG(logits && labels && loss_sum && n > 0 && h > 0 && w > 0 && c > 0, "ce_logits: bad args");
+  T2H_CHECK_ARG(c_pad >= c && c_pad % 8 == 0 && c_pad <= 256, "ce_logits: c=%d c_pad=%d", c, c_pad);
+  T2H_CHECK_ARG(!grad_planes || terms == 1 || terms == 2, "ce_logits: terms=%d", terms);
+  const long long npix = (long long)n * h * w;
+  int g = 1;
+  while (g < c_pad / 8) g <<= 1;
+  const int block = 256;
+  ce_logits_kernel<<<grid_cap(npix, block / g, 4), block, c_pad * sizeof(double), as_stream(stream)>>>(
+      logits, reinterpret_cast<const long long*>(labels), npix, c, c_pad, g, gscale, loss_sum,
+      reinterpret_cast<__half*>(grad_planes), terms, colsum);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_shape_attr_embed_bwd(const int64_t* attr, const int32_t* cls_off, const float* w1t, const float* b1,
+                             const float* w2, const float* b2, const float* wf1, const float* bf1, const float* wf2,
+                             const float* bf2, const float* d_out, float* grad, const int64_t* goff, int b,
+                             int n_attr, int dim, int out_dim, t2h_stream_t stream) {
+  T2H_CHECK_ARG(attr && cls_off && w1t && b1 && w2 && b2 && wf1 && bf1 && wf2 && bf2 && d_out && grad && goff,
+                "shape_attr_embed_bwd: null operand");
+  T2H_CHECK_ARG(b > 0 && n_attr > 0 && dim > 0 && out_dim > 0, "shape_attr_embed_bwd: bad shape");
+  const size_t smem = (size_t)(4 * n_attr * dim + 3 * out_dim) * sizeof(float);
+  T2H_CHECK_ARG(smem <= 48 * 1024, "shape_attr_embed_bwd: n_attr*dim=%d, out_dim=%d too large", n_attr * dim,
+                out_dim);
+  shape_attr_embed_bwd_kernel<<<1, 512, smem, as_stream(stream)>>>(
+      reinterpret_cast<const long long*>(attr), cls_off, w1t, b1, w2, b2, wf1, bf1, wf2, bf2, d_out, grad,
+      reinterpret_cast<const long long*>(goff), b, n_attr, dim, out_dim);
   T2H_LAUNCH_OK();
   return T2H_OK;
 }

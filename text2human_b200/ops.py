@@ -1102,7 +1102,7 @@ def conv_wgrad(dy, x, taps, dw, *, n, alpha=1.0, k_split=0):
     return dw
 
 
-ACT_CODE = {None: 0, "none": 0, "swish": 1, "lrelu": 2}
+ACT_CODE = {None: 0, "none": 0, "swish": 1, "lrelu": 2, "relu": 3}
 
 
 def norm_apply(x, stats, gamma, beta, *, act, groups, eps, n=None, terms=None):
@@ -1131,12 +1131,13 @@ def norm_stats(x, groups, n=None):
 
 
 def norm_bwd(x, stats, gamma, beta, dy, *, act, groups, eps, dgamma=None, dbeta=None, add=None, want_planes=False,
-             n=None, terms=None, colsum_out=None, want_dx=True, sums=None):
+             n=None, terms=None, colsum_out=None, want_dx=True, sums=None, dy_scale=None):
     """backward of act(norm(x)*gamma+beta): -> dx fp32 (+ add) [, planes of dx]; dgamma/dbeta accumulated;
     ``colsum_out`` [C] += column sums of dx (the bias gradient of the conv that produced x); ``want_dx=False``
     (with ``want_planes``) skips the fp32 copy when only the conv gradients consume dx (4 of 14 B per element);
     ``sums``: pass 1's result from ``nb_context`` (the data-gradient conv accumulated it in its epilogue) -- the
-    reduce launch and its 8 B per element are skipped"""
+    reduce launch and its 8 B per element are skipped; ``dy_scale`` fp32 [N,C]: dy is first multiplied by the factor of
+    its image and channel (a Dropout2d between the activation and its consumer; not with add / colsum_out / sums)"""
     _need_cuda(x, dy)
     N, H, W, Cc = x.shape
     terms = terms or get_terms()
@@ -1150,6 +1151,14 @@ def norm_bwd(x, stats, gamma, beta, dy, *, act, groups, eps, dgamma=None, dbeta=
     else:
         ws = torch.empty((nn_ * Cc * 2,), dtype=torch.float64, device=x.device)
     assert dy.is_contiguous() and x.is_contiguous() and (add is None or add.is_contiguous())
+    if dy_scale is not None:
+        assert add is None and colsum_out is None and sums is None
+        _count(3)
+        _lib.check(_lib.load().t2h_norm_bwd_drop(_ptr(x), _ptr(stats), _ptr(gamma), _ptr(beta), _ptr(dy),
+                                                 _ptr(_f32c(dy_scale)), H * W, _ptr(dx), _ptr(planes), terms,
+                                                 _ptr(dgamma), _ptr(dbeta), _ptr(ws), nn_, hw, Cc, groups, eps,
+                                                 ACT_CODE[act], _stream()))
+        return (dx, planes) if want_planes else dx
     _count(3 if sums is None else 2)
     _lib.check(_lib.load().t2h_norm_bwd(_ptr(x), _ptr(stats), _ptr(gamma), _ptr(beta), _ptr(dy), _ptr(add), _ptr(dx),
                                         _ptr(planes), terms, _ptr(dgamma), _ptr(dbeta), _ptr(ws), nn_, hw, Cc, groups,
@@ -1299,3 +1308,111 @@ def sample_step(logits_own, u, tex, x_t, unmasked, *, t, temp, seed, step, n_hea
     _lib.check(_lib.load().t2h_sample_step(_ptr(logits_own), _ptr(u), _ptr(tex), _ptr(x_t), _ptr(unmasked), M, ncls,
                                            n_heads, 1.0 / float(t), 1.0 / float(temp), int(seed), int(step), cont_stride,
                                            _stream()))
+
+
+# ----------------------------------------------------------------------------
+# parsing-generator training (ParsingGenModel.optimize_parameters): norm apply with an fp32 output and a Dropout2d
+# factor, max-pool + broadcast-concat backward, bilinear x2 backward, pixel cross-entropy, ShapeAttrEmbedding backward
+# ----------------------------------------------------------------------------
+def norm_apply_ex(x, stats, gamma, beta, *, act, groups, eps, n=None, drop=None, want_f32=True, want_planes=False,
+                  terms=None):
+    """act(norm(x)*gamma+beta) [* drop[image, channel]] of fp32 NHWC x [N,H,W,C] -> (fp32 NHWC or None, planes or
+    None); ``n`` / ``groups`` as norm_apply (BatchNorm2d in training mode: n=1, groups=C); ``drop`` fp32 [N,C]"""
+    _need_cuda(x)
+    N, H, W, Cc = x.shape
+    assert want_f32 or want_planes
+    terms = terms or get_terms()
+    nn_, hw = (N, H * W) if n is None else (n, N * H * W // n)
+    out = torch.empty_like(x) if want_f32 else None
+    planes = torch.empty((terms, N, H, W, Cc), dtype=torch.float16, device=x.device) if want_planes else None
+    if drop is not None:
+        assert drop.shape == (N, Cc), (drop.shape, x.shape)
+        drop = _f32c(drop)
+    _count(1)
+    _lib.check(_lib.load().t2h_norm_apply_ex(_ptr(x), _ptr(stats), _ptr(_f32c(gamma)), _ptr(_f32c(beta)), _ptr(drop),
+                                             H * W, _ptr(out), _ptr(planes), nn_, hw, Cc, groups, eps, ACT_CODE[act],
+                                             terms, _stream()))
+    return out, planes
+
+
+def maxpool2_bcast_bwd(da, c, c_e, *, x=None, dx=None, de=None, pool=True, in_hw=None, accumulate=False):
+    """Backward of [MaxPool2d(2) of] cat([x, e broadcast over H, W]) (a ShapeUNet encoder stage's operand).
+    da fp32 [N,h,w,ld] (the data-gradient conv's output, channels [0,c) x, [c,c+c_e) e).  ``dx`` fp32 [N,H,W,c]
+    (or None): the x part routed to the first maximum of each window of the saved pre-pool ``x``; ``de`` fp32
+    [N,c_e] (or None): the per-image sums of the e channels, fixed order.  Both written, or added with
+    ``accumulate``.  ``in_hw``: (H, W) of x (default: twice da's with pool)."""
+    _need_cuda(da)
+    N, h, w, ld = da.shape
+    assert da.is_contiguous() and da.dtype == torch.float32 and ld >= c + c_e
+    H, W = in_hw if in_hw is not None else ((2 * h, 2 * w) if pool else (h, w))
+    if dx is not None:
+        assert dx.shape == (N, H, W, c) and dx.is_contiguous() and (not pool or x.shape == dx.shape)
+        _need_cuda(dx, x)
+    ws = None
+    if de is not None and c_e:
+        assert de.shape == (N, c_e) and de.is_contiguous()
+        ws = torch.empty((N * 32 * c_e,), dtype=torch.float32, device=da.device)
+    _count((dx is not None) + 2 * (ws is not None))
+    _lib.check(_lib.load().t2h_maxpool2_bcast_bwd(_ptr(da), ld, _ptr(x), _ptr(dx), 1 if accumulate else 0, _ptr(de),
+                                                  _ptr(ws), N, H, W, c, c_e if ws is not None else 0,
+                                                  1 if pool else 0, _stream()))
+    return dx, de
+
+
+def bilinear2x_bwd(dy):
+    """adjoint of the bilinear x2 upsample (align_corners=False): fp32 [N,2H,2W,C] -> [N,H,W,C]"""
+    _need_cuda(dy)
+    N, H2, W2, Cc = dy.shape
+    assert dy.is_contiguous() and dy.dtype == torch.float32
+    out = torch.empty((N, H2 // 2, W2 // 2, Cc), dtype=torch.float32, device=dy.device)
+    _count(1)
+    _lib.check(_lib.load().t2h_bilinear2x_bwd(_ptr(dy), _ptr(out), N, H2 // 2, W2 // 2, Cc, _stream()))
+    return out
+
+
+def check_labels(labels, n_classes, ignore_index=-100):
+    """raise ValueError for a label outside [0, n_classes) that is not ``ignore_index`` (F.cross_entropy rejects
+    those too); one device->host read"""
+    if labels.dtype.is_floating_point or labels.dtype == torch.bool:
+        raise ValueError(f"class labels must be integers, got {labels.dtype}")
+    bad = (labels != ignore_index) & ((labels < 0) | (labels >= n_classes))
+    if bool(bad.any()):
+        v = int(labels[bad].reshape(-1)[0])
+        raise ValueError(f"class label {v} is outside 0..{n_classes - 1} and is not ignore_index ({ignore_index})")
+
+
+def ce_logits(logits, labels, sum_out, gscale=1.0, want_grad=True, colsum_out=None, terms=None, checked=False):
+    """Pixel cross-entropy of fp32 NHWC ``logits`` [N,H,W,C] against int64 ``labels`` [N,H,W] (checked on the host
+    first, see check_labels): sum_out[0] += the loss summed over the labelled pixels; -> fp16 planes
+    [T,N,H,W,c_pad] of gscale * (softmax(logits) - onehot), 0 on ignored pixels (or None); ``colsum_out`` [C] += the
+    column sums of that gradient.  ``checked``: the caller already ran check_labels (ignore_index -100)"""
+    _need_cuda(logits, labels, sum_out)
+    N, H, W, Cc = logits.shape
+    assert logits.is_contiguous() and logits.dtype == torch.float32 and labels.numel() == N * H * W
+    assert sum_out.dtype == torch.float64 and (colsum_out is None or colsum_out.numel() == Cc)
+    if not checked:
+        check_labels(labels, Cc)
+    labels = labels.to(torch.int64).contiguous()
+    terms = terms or get_terms()
+    cp = (Cc + 7) // 8 * 8
+    planes = torch.empty((terms, N, H, W, cp), dtype=torch.float16, device=logits.device) if want_grad else None
+    _count(1)
+    _lib.check(_lib.load().t2h_ce_logits(_ptr(logits), _ptr(labels), N, H, W, Cc, cp, gscale, _ptr(sum_out),
+                                         _ptr(planes), terms, _ptr(colsum_out), _stream()))
+    return planes
+
+
+def shape_attr_embed_bwd(attr, packed, d_out, grad, goff):
+    """ShapeAttrEmbedding backward: every parameter gradient += from d_out fp32 [B,out_dim], into the flat fp32
+    buffer ``grad`` at the int64 element offsets ``goff`` [(n_attr+1)*4] (see t2h_shape_attr_embed_bwd); attr
+    already range-checked"""
+    p = packed
+    _need_cuda(attr, d_out, grad, goff)
+    attr = attr.to(torch.int64).contiguous()
+    B, A = attr.shape
+    D, O = p["b1"].shape[1], p["bf1"].shape[0]
+    assert d_out.shape == (B, O) and d_out.is_contiguous() and goff.numel() == 4 * (A + 1)
+    _count(1)
+    _lib.check(_lib.load().t2h_shape_attr_embed_bwd(
+        _ptr(attr), _ptr(p["cls_off"]), _ptr(p["w1t"]), _ptr(p["b1"]), _ptr(p["w2"]), _ptr(p["b2"]), _ptr(p["wf1"]),
+        _ptr(p["bf1"]), _ptr(p["wf2"]), _ptr(p["bf2"]), _ptr(d_out), _ptr(grad), _ptr(goff), B, A, D, O, _stream()))
