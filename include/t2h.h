@@ -537,6 +537,21 @@ int t2h_shape_attr_embed_bwd(const int64_t* attr, const int32_t* cls_off, const 
                              const float* bf2, const float* d_out, float* grad, const int64_t* goff, int b,
                              int n_attr, int dim, int out_dim, t2h_stream_t stream);
 
+/* ------------------------------------------------------------------------
+ * Training the index-prediction heads (VQGANTextureAwareSpatialHierarchyInferenceModel.optimize_parameters,
+ * hierarchy_inference_model.py:227-245)
+ * ---------------------------------------------------------------------- */
+/* The 18 heads' conv_seg + CrossEntropyLoss(ignore_index=-1) summed over heads, routed: position m (of m rows) has a
+ * target only in head k = tex[m], class t = own[m].  y fp32 [m][g*c] (the heads' Dropout2d outputs, head-major
+ * channels), w fp32 [g][ncls][c], bias [g][ncls].  For each row with k in [0,g) and t in [0,ncls):
+ * loss_sum[0] += logsumexp(l) - l[t] with l = w[k] y[m][k*c..] + bias[k] (fp32 FMA); dl = gscale (softmax(l) -
+ * onehot_t); dy[m][k*c..] = dl w[k]; dw[k] += dl^T y[m][k*c..] and db[k] += dl (fixed-order sums over the head's
+ * rows in row order, no atomics).  Every other dy element is written 0 (all of a row without a target).
+ * Workspace: order int32 [m], off int32 [g+2], dl fp32 [m][ncls].  c % 8 == 0, 8 <= c <= 512, g < 64. */
+int t2h_routed_head_ce(const float* y, const int64_t* tex, const int64_t* own, const float* w, const float* bias,
+                       int64_t m, int g, int c, int ncls, float gscale, double* loss_sum, float* dy, float* dw,
+                       float* db, int32_t* order, int32_t* off, float* dl, t2h_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1004,6 +1004,241 @@ __global__ void shape_attr_embed_bwd_kernel(const long long* __restrict__ attr, 
   }
 }
 
+// ---- routed multi-head cross-entropy (MultiHeadFCNHead + 18 CrossEntropyLoss(ignore_index=-1),
+// hierarchy_inference_model.py:227-245): only the head of a position's own texture has a target there, so each
+// position computes that one head's logits.  Rows are grouped by head with a stable counting sort; a row tile of
+// one head stages that head's weights in shared memory chunk by chunk; the weight / bias gradients are fixed-order
+// sums over the head's rows (no floating-point atomics, bitwise reproducible).
+constexpr int kRouteMaxBins = 64;   // heads + the bin of rows without a target
+constexpr int kRouteThreads = 256;
+constexpr int kRouteOut = 2048;     // outputs per CTA (rows x channels, classes x channels): 8 per thread
+constexpr int kRouteCls = 32;       // classes per staged weight chunk
+constexpr int kRouteRB = 16;        // rows per staged chunk of the weight gradient
+
+__device__ __forceinline__ int route_bin(const long long* __restrict__ tex, const long long* __restrict__ own,
+                                         int r, int G, int ncls) {
+  const long long k = tex[r], t = own[r];
+  return (k >= 0 && k < G && t >= 0 && t < ncls) ? (int)k : G;
+}
+
+// stable counting sort of the rows by bin (one CTA of 1024 threads): order[slot] = row, off[b] = first slot of bin
+// b (b = G: rows without a target), off[G+1] = M.  Within a 1024-row tile, a row's rank among the rows of its bin
+// comes from __match_any_sync and per-warp counts, so rows keep their index order inside each bin.
+__global__ void __launch_bounds__(1024) route_sort_kernel(const long long* __restrict__ tex,
+                                                          const long long* __restrict__ own, int M, int G, int ncls,
+                                                          int* __restrict__ order, int* __restrict__ off) {
+  __shared__ int cnt[kRouteMaxBins], base[kRouteMaxBins];
+  __shared__ int wc[32][kRouteMaxBins + 1];
+  const int nb = G + 1, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int b = threadIdx.x; b < nb; b += blockDim.x) cnt[b] = 0;
+  __syncthreads();
+  for (int r = threadIdx.x; r < M; r += blockDim.x) atomicAdd(&cnt[route_bin(tex, own, r, G, ncls)], 1);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int s = 0;
+    for (int b = 0; b < nb; ++b) {
+      base[b] = off[b] = s;
+      s += cnt[b];
+    }
+    off[nb] = s;
+  }
+  __syncthreads();
+  for (int t0 = 0; t0 < M; t0 += blockDim.x) {
+    const int r = t0 + threadIdx.x;
+    const int k = r < M ? route_bin(tex, own, r, G, ncls) : nb;  // nb: past the end, never stored
+    for (int i = threadIdx.x; i < 32 * (kRouteMaxBins + 1); i += blockDim.x) (&wc[0][0])[i] = 0;
+    __syncthreads();
+    const unsigned same = __match_any_sync(0xffffffffu, k);
+    const int rank = __popc(same & ((1u << lane) - 1u));
+    if (rank == 0) wc[warp][k] = __popc(same);
+    __syncthreads();
+    for (int b = threadIdx.x; b < nb; b += blockDim.x) {  // exclusive scan over the warps, per bin
+      int s = 0;
+      for (int w = 0; w < 32; ++w) {
+        const int c = wc[w][b];
+        wc[w][b] = s;
+        s += c;
+      }
+      cnt[b] = s;
+    }
+    __syncthreads();
+    if (r < M) order[base[k] + wc[warp][k] + rank] = r;
+    __syncthreads();
+    for (int b = threadIdx.x; b < nb; b += blockDim.x) base[b] += cnt[b];
+    __syncthreads();
+  }
+}
+
+// One CTA = up to R slots of one bin (R * C <= kRouteOut).  For head k: logits = W_k y + b_k into dl (slot-major
+// [M][ncls]), then per row (one warp) loss += logsumexp - logit_t and dl = gscale (softmax - onehot_t), then
+// dy[row][k*C..] = dl W_k and every other channel of the row 0.  Bin G rows get an all-zero dy row.
+__global__ void __launch_bounds__(kRouteThreads) route_rows_kernel(
+    const float* __restrict__ y, const float* __restrict__ w, const float* __restrict__ bias,
+    const long long* __restrict__ own, const int* __restrict__ order, const int* __restrict__ off, int G, int C,
+    int ncls, int R, float gscale, double* __restrict__ loss, float* __restrict__ dl, float* __restrict__ dy) {
+  extern __shared__ float rsm[];
+  const int ld = C + 1;              // odd row pitch: a warp reading one channel of 32 classes is conflict-free
+  float* ys = rsm;                   // [R][ld]  the tile's rows of the head's C channels
+  float* ws = ys + R * ld;           // [kRouteCls][ld]  a chunk of W_k
+  float* ds = ws + kRouteCls * ld;   // [R][kRouteCls]   the same chunk of dl
+  int t = blockIdx.x, k = -1, s0 = 0, n = 0;
+  for (int b = 0; b <= G; ++b) {
+    const int nb = off[b + 1] - off[b], tiles = (nb + R - 1) / R;
+    if (t < tiles) {
+      k = b;
+      s0 = off[b] + t * R;
+      n = min(R, nb - t * R);
+      break;
+    }
+    t -= tiles;
+  }
+  if (k < 0) return;  // grid upper bound: no tile left (uniform over the CTA)
+  const long long GC = (long long)G * C;
+  if (k == G) {
+    for (long long i = threadIdx.x; i < n * GC; i += blockDim.x) {
+      const int r = (int)(i / GC);
+      dy[(long long)order[s0 + r] * GC + (i - r * GC)] = 0.f;
+    }
+    return;
+  }
+  const float* wk = w + (long long)k * ncls * C;
+  const float* bk = bias + (long long)k * ncls;
+  for (int i = threadIdx.x; i < R * C; i += blockDim.x) {
+    const int r = i / C, j = i - r * C;
+    ys[r * ld + j] = r < n ? y[(long long)order[s0 + r] * GC + (long long)k * C + j] : 0.f;
+  }
+  for (int c0 = 0; c0 < ncls; c0 += kRouteCls) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < kRouteCls * C; i += blockDim.x) {
+      const int cc = i / C, j = i - cc * C;
+      ws[cc * ld + j] = c0 + cc < ncls ? wk[(long long)(c0 + cc) * C + j] : 0.f;
+    }
+    __syncthreads();
+    for (int p = threadIdx.x; p < n * kRouteCls; p += blockDim.x) {
+      const int r = p / kRouteCls, cc = p - r * kRouteCls;
+      if (c0 + cc >= ncls) continue;
+      const float* yr = ys + r * ld;
+      const float* wr = ws + cc * ld;
+      float s = 0.f;
+      for (int j = 0; j < C; ++j) s = fmaf(wr[j], yr[j], s);
+      dl[(long long)(s0 + r) * ncls + c0 + cc] = s + bk[c0 + cc];
+    }
+  }
+  __syncthreads();
+  const int lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  double acc = 0.0;
+  for (int r = threadIdx.x >> 5; r < n; r += nw) {
+    float* row = dl + (long long)(s0 + r) * ncls;
+    const int tgt = (int)own[order[s0 + r]];
+    float m = -INFINITY;
+    for (int c = lane; c < ncls; c += 32) m = fmaxf(m, row[c]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    float s = 0.f;
+    for (int c = lane; c < ncls; c += 32) s += expf(row[c] - m);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    const float xt = row[tgt];
+    __syncwarp();  // every lane has read the target logit before any lane overwrites the row
+    if (lane == 0) acc += (double)(m + logf(s) - xt);
+    const float inv = 1.f / s;
+    for (int c = lane; c < ncls; c += 32) row[c] = gscale * (expf(row[c] - m) * inv - (c == tgt ? 1.f : 0.f));
+  }
+  float a[kRouteOut / kRouteThreads];
+#pragma unroll
+  for (int e = 0; e < kRouteOut / kRouteThreads; ++e) a[e] = 0.f;
+  for (int c0 = 0; c0 < ncls; c0 += kRouteCls) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < kRouteCls * C; i += blockDim.x) {
+      const int cc = i / C, j = i - cc * C;
+      ws[cc * ld + j] = c0 + cc < ncls ? wk[(long long)(c0 + cc) * C + j] : 0.f;
+    }
+    for (int i = threadIdx.x; i < R * kRouteCls; i += blockDim.x) {
+      const int r = i / kRouteCls, cc = i - r * kRouteCls;
+      ds[i] = (r < n && c0 + cc < ncls) ? dl[(long long)(s0 + r) * ncls + c0 + cc] : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int e = 0; e < kRouteOut / kRouteThreads; ++e) {
+      const int p = threadIdx.x + e * kRouteThreads;
+      if (p < R * C) {
+        const int r = p / C, j = p - r * C;
+        float s = a[e];
+        for (int cc = 0; cc < kRouteCls; ++cc) s = fmaf(ds[r * kRouteCls + cc], ws[cc * ld + j], s);
+        a[e] = s;
+      }
+    }
+  }
+#pragma unroll
+  for (int e = 0; e < kRouteOut / kRouteThreads; ++e) {
+    const int p = threadIdx.x + e * kRouteThreads;
+    if (p < n * C) {
+      const int r = p / C, j = p - r * C;
+      dy[(long long)order[s0 + r] * GC + (long long)k * C + j] = a[e];
+    }
+  }
+  for (long long i = threadIdx.x; i < n * GC; i += blockDim.x) {
+    const int r = (int)(i / GC);
+    const long long q = i - r * GC;
+    if (q / C != k) dy[(long long)order[s0 + r] * GC + q] = 0.f;
+  }
+  block_add(acc, loss);
+}
+
+// grid (classes / CB, G), CB * C <= kRouteOut: dw[k][c][:] += sum over the head's slots (in slot order) of
+// dl[slot][c] y[row][k*C..], db[k][c] += sum of dl[slot][c]; a head without rows adds exact zeros
+__global__ void __launch_bounds__(kRouteThreads) route_wgrad_kernel(
+    const float* __restrict__ y, const int* __restrict__ order, const int* __restrict__ off,
+    const float* __restrict__ dl, int G, int C, int ncls, int CB, float* __restrict__ dw, float* __restrict__ db) {
+  extern __shared__ float wsm[];
+  float* ds = wsm;                 // [kRouteRB][CB]
+  float* ys = ds + kRouteRB * CB;  // [kRouteRB][C]
+  const int k = blockIdx.y, c0 = blockIdx.x * CB;
+  const int nc = min(CB, ncls - c0);
+  const int s_beg = off[k], s_end = off[k + 1];
+  const long long GC = (long long)G * C;
+  float a[kRouteOut / kRouteThreads];
+#pragma unroll
+  for (int e = 0; e < kRouteOut / kRouteThreads; ++e) a[e] = 0.f;
+  float sb = 0.f;
+  for (int s = s_beg; s < s_end; s += kRouteRB) {
+    const int nr = min(kRouteRB, s_end - s);
+    __syncthreads();
+    for (int i = threadIdx.x; i < kRouteRB * CB; i += blockDim.x) {
+      const int r = i / CB, cc = i - r * CB;
+      ds[i] = (r < nr && cc < nc) ? dl[(long long)(s + r) * ncls + c0 + cc] : 0.f;
+    }
+    for (int i = threadIdx.x; i < kRouteRB * C; i += blockDim.x) {
+      const int r = i / C, j = i - r * C;
+      ys[i] = r < nr ? y[(long long)order[s + r] * GC + (long long)k * C + j] : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int e = 0; e < kRouteOut / kRouteThreads; ++e) {
+      const int p = threadIdx.x + e * kRouteThreads;
+      if (p < CB * C) {
+        const int cc = p / C, j = p - cc * C;
+        float v = a[e];
+#pragma unroll 4
+        for (int r = 0; r < kRouteRB; ++r) v = fmaf(ds[r * CB + cc], ys[r * C + j], v);
+        a[e] = v;
+      }
+    }
+    if (threadIdx.x < CB) {
+      for (int r = 0; r < kRouteRB; ++r) sb += ds[r * CB + threadIdx.x];
+    }
+  }
+#pragma unroll
+  for (int e = 0; e < kRouteOut / kRouteThreads; ++e) {
+    const int p = threadIdx.x + e * kRouteThreads;
+    if (p < nc * C) {
+      const int cc = p / C, j = p - cc * C;
+      dw[((long long)k * ncls + c0 + cc) * C + j] += a[e];
+    }
+  }
+  if (threadIdx.x < nc) db[(long long)k * ncls + c0 + threadIdx.x] += sb;
+}
+
 }  // namespace t2h
 
 using namespace t2h;
@@ -1248,6 +1483,34 @@ int t2h_shape_attr_embed_bwd(const int64_t* attr, const int32_t* cls_off, const 
   shape_attr_embed_bwd_kernel<<<1, 512, smem, as_stream(stream)>>>(
       reinterpret_cast<const long long*>(attr), cls_off, w1t, b1, w2, b2, wf1, bf1, wf2, bf2, d_out, grad,
       reinterpret_cast<const long long*>(goff), b, n_attr, dim, out_dim);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+// ---- index-prediction training (VQGANTextureAwareSpatialHierarchyInferenceModel.optimize_parameters)
+int t2h_routed_head_ce(const float* y, const int64_t* tex, const int64_t* own, const float* w, const float* bias,
+                       int64_t m, int g, int c, int ncls, float gscale, double* loss_sum, float* dy, float* dw,
+                       float* db, int32_t* order, int32_t* off, float* dl, t2h_stream_t stream) {
+  T2H_CHECK_ARG(y && tex && own && w && bias && loss_sum && dy && dw && db && order && off && dl,
+                "routed_head_ce: null operand");
+  T2H_CHECK_ARG(m > 0 && m <= 0x7fffffffLL && g >= 1 && g < kRouteMaxBins && ncls > 0,
+                "routed_head_ce: m=%lld g=%d ncls=%d unsupported", (long long)m, g, ncls);
+  T2H_CHECK_ARG(c >= 8 && c % 8 == 0 && c <= 512, "routed_head_ce: c=%d (a multiple of 8, at most 512)", c);
+  cudaStream_t st = as_stream(stream);
+  const int M = (int)m;
+  route_sort_kernel<<<1, 1024, 0, st>>>(reinterpret_cast<const long long*>(tex),
+                                        reinterpret_cast<const long long*>(own), M, g, ncls, order, off);
+  T2H_LAUNCH_OK();
+  const int R = min(64, kRouteOut / c);
+  const size_t smem = (size_t)((R + kRouteCls) * (c + 1) + R * kRouteCls) * sizeof(float);
+  if (smem > 48 * 1024)
+    T2H_CUDA(cudaFuncSetAttribute(route_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  route_rows_kernel<<<(unsigned)(ceil_div64(m, R) + g + 1), kRouteThreads, smem, st>>>(
+      y, w, bias, reinterpret_cast<const long long*>(own), order, off, g, c, ncls, R, gscale, loss_sum, dl, dy);
+  T2H_LAUNCH_OK();
+  const int CB = kRouteOut / c;
+  route_wgrad_kernel<<<dim3(ceil_div(ncls, CB), g), kRouteThreads, (size_t)kRouteRB * (CB + c) * sizeof(float),
+                       st>>>(y, order, off, dl, g, c, ncls, CB, dw, db);
   T2H_LAUNCH_OK();
   return T2H_OK;
 }

@@ -21,13 +21,27 @@ class ConvP:
     __slots__ = ("mod", "k", "co", "ci", "co_p", "ci_p", "w", "gw", "b", "gb", "wn", "wt")
 
 
+class ConvStack:
+    """Convolutions of equal shape that always run as ONE convolution with their outputs stacked along the output
+    channels (the index-prediction heads' 3x3 ConvModules).  ParamSpace keeps their weights as one tap-major block
+    ``[K*K, n*Cout, Cin]``, so the stacked forward operand and weight gradient need no per-step copy; each member's
+    ``weight`` / ``.grad`` is a view of its ``Cout``-row slice.  ``done(stack)`` reports the whole block."""
+
+    def __init__(self, convs):
+        self.convs = tuple(convs)
+        co, ci, kh, kw = self.convs[0].weight.shape
+        assert kh == kw and co % 8 == 0 and ci % 8 == 0, "stacked convs need channel counts that are multiples of 8"
+        assert all(tuple(c.weight.shape) == (co, ci, kh, kw) and c.bias is None for c in self.convs)
+
+
 class ParamSpace:
     """Flat fp32 parameter / gradient / Adam-moment buffers for ``order``, modules in backward-completion order.
 
     A Conv2d's weight is kept TAP-MAJOR ``[K*K, Cout_p, Cin_p]`` (the layout the kernels' packed operands and the
     weight-gradient kernel's output share) and the conv gets a ``ConvP`` in ``convs``.  A tuple of Conv2d or Linear
     modules is one group laid out weights first, then biases, so that a fused projection (q | k | v, the sampler's
-    18 heads) reads them as one matrix (``joint``); a conv alone is a group of one.  Any other module contributes its
+    18 heads) reads them as one matrix (``joint``); a conv alone is a group of one; a tuple of BatchNorm2d is one
+    group too (gammas back to back, then betas).  A ``ConvStack`` is one conv of ``n*Cout`` output channels.  Any other module contributes its
     own parameters (``parameters(recurse=False)``).  Every slot starts 32-byte aligned.
 
     A gradient bucket closes after the module (a group: its last member) that brings it to ``bucket_bytes`` or more,
@@ -48,7 +62,14 @@ class ParamSpace:
         for mod in order:
             start = total
             group = mod if isinstance(mod, tuple) else (mod,)
-            if isinstance(mod, (tuple, nn.Conv2d)):
+            if isinstance(mod, ConvStack):
+                co, ci, k, _ = mod.convs[0].weight.shape
+                cp = ConvP()
+                cp.mod, cp.k, cp.co, cp.ci = mod, k, co * len(mod.convs), ci
+                cp.co_p, cp.ci_p = cp.co, cp.ci
+                take(mod.convs[0].weight, k * k * cp.co * cp.ci, ("stack", cp))
+                self.convs[mod] = cp
+            elif isinstance(mod, (tuple, nn.Conv2d)):
                 for m_ in group:
                     if isinstance(m_, nn.Conv2d):
                         co, ci, kh, kw = m_.weight.shape
@@ -76,6 +97,20 @@ class ParamSpace:
         self.gview = {}
         with torch.no_grad():
             for p, off, tag in self.slots:
+                if isinstance(tag, tuple) and tag[0] == "stack":
+                    cp = tag[1]
+                    n = cp.k * cp.k * cp.co * cp.ci
+                    cp.w = self.flat_p[off:off + n].view(cp.k * cp.k, cp.co, cp.ci)
+                    cp.gw = self.flat_g[off:off + n].view(cp.k * cp.k, cp.co, cp.ci)
+                    cp.b = cp.gb = None
+                    per = cp.co // len(cp.mod.convs)
+                    for j, c in enumerate(cp.mod.convs):
+                        rows = slice(j * per, (j + 1) * per)
+                        cp.w[:, rows].copy_(G.oihw_to_master(c.weight.detach().to(device)))
+                        c.weight.data = G.master_as_oihw(cp.w[:, rows], per, cp.ci, cp.k)
+                        c.weight.grad = G.master_as_oihw(cp.gw[:, rows], per, cp.ci, cp.k)
+                        self.gview[id(c.weight)] = c.weight.grad
+                    continue
                 if isinstance(tag, ConvP):
                     cp = tag
                     n = cp.k * cp.k * cp.co_p * cp.ci_p

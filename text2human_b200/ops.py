@@ -1416,3 +1416,47 @@ def shape_attr_embed_bwd(attr, packed, d_out, grad, goff):
     _lib.check(_lib.load().t2h_shape_attr_embed_bwd(
         _ptr(attr), _ptr(p["cls_off"]), _ptr(p["w1t"]), _ptr(p["b1"]), _ptr(p["w2"]), _ptr(p["b2"]), _ptr(p["wf1"]),
         _ptr(p["bf1"]), _ptr(p["wf2"]), _ptr(p["bf2"]), _ptr(d_out), _ptr(grad), _ptr(goff), B, A, D, O, _stream()))
+
+
+# ----------------------------------------------------------------------------
+# index-prediction training: the 18 heads' conv_seg + cross-entropy, routed to each position's own head
+# ----------------------------------------------------------------------------
+def check_routed_targets(tex, own, n_heads, n_classes, ignore_index=-1):
+    """raise ValueError for a position whose head id ``tex`` lies in [0, n_heads) and whose class ``own`` is neither
+    in [0, n_classes) nor ``ignore_index`` (F.cross_entropy rejects it); one device->host read"""
+    for name, t in (("texture ids", tex), ("targets", own)):
+        if t.dtype.is_floating_point or t.dtype == torch.bool:
+            raise ValueError(f"{name} must be integers, got {t.dtype}")
+    if tex.shape != own.shape:
+        raise ValueError(f"texture ids {tuple(tex.shape)} and targets {tuple(own.shape)} differ in shape")
+    live = (tex >= 0) & (tex < n_heads)
+    bad = live & (own != ignore_index) & ((own < 0) | (own >= n_classes))
+    if bool(bad.any()):
+        v = int(own[bad].reshape(-1)[0])
+        raise ValueError(f"target {v} is outside 0..{n_classes - 1} and is not ignore_index ({ignore_index})")
+
+
+def routed_head_ce(y, tex, own, w, b, loss_sum, dw, db, gscale=1.0):
+    """Sum over heads of the cross-entropy of ``n_heads`` 1x1 conv_seg heads, each position scored only by its own
+    head (see t2h_routed_head_ce).  y fp32 [M, G*C] (head-major channels), tex / own int64 [M] (a position whose head
+    id is outside [0, G), or whose target is outside [0, ncls), has no target), w fp32 [G, ncls, C], b [G, ncls].
+    loss_sum[0] += the summed loss; dw / db (views into the flat gradient store) += the heads' gradients scaled by
+    ``gscale``; -> dy fp32 [M, G*C], the gradient of y (zero outside each position's own head)."""
+    _need_cuda(y, tex, own, w, b, loss_sum, dw, db)
+    M, GC = y.shape
+    G, ncls, Cc = w.shape
+    assert GC == G * Cc and y.is_contiguous() and y.dtype == torch.float32
+    assert w.is_contiguous() and b.shape == (G, ncls) and b.is_contiguous() and loss_sum.dtype == torch.float64
+    assert dw.shape == w.shape and dw.is_contiguous() and db.shape == b.shape and db.is_contiguous()
+    tex = tex.reshape(-1).to(torch.int64).contiguous()
+    own = own.reshape(-1).to(torch.int64).contiguous()
+    assert tex.numel() == M and own.numel() == M
+    dy = torch.empty_like(y)
+    order = torch.empty((M,), dtype=torch.int32, device=y.device)
+    off = torch.empty((G + 2,), dtype=torch.int32, device=y.device)
+    dl = torch.empty((M, ncls), dtype=torch.float32, device=y.device)
+    _count(3)
+    _lib.check(_lib.load().t2h_routed_head_ce(_ptr(y), _ptr(tex), _ptr(own), _ptr(w), _ptr(b), M, G, Cc, ncls,
+                                              gscale, _ptr(loss_sum), _ptr(dy), _ptr(dw), _ptr(db), _ptr(order),
+                                              _ptr(off), _ptr(dl), _stream()))
+    return dy

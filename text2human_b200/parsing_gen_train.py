@@ -116,10 +116,11 @@ class ConvModuleL(Layer):
 
 class BasicConvBlockL:
     """BasicConvBlock (unet_arch.py:113-181): ConvModules in sequence; the last one's output is fp32 NHWC (it feeds a
-    pooling / upsampling conversion or a skip connection)"""
+    pooling / upsampling conversion or a skip connection).  ``need_dx=False``: the block's input is constant (a
+    frozen feature map), so its first conv computes no data gradient and ``bwd`` returns None."""
 
-    def __init__(self, tr, blk):
-        self.convs = [ConvModuleL(tr, c) for c in blk.convs]
+    def __init__(self, tr, blk, need_dx=True):
+        self.convs = [ConvModuleL(tr, c, need_dx=need_dx or i > 0) for i, c in enumerate(blk.convs)]
 
     def fwd(self, a):
         n = len(self.convs)
@@ -159,9 +160,16 @@ def unet_decode_layers(tr, decoder):
 
 def backward_order(embedder, unet, head):
     """the parameter-holding modules in the order the backward pass finishes their gradients"""
+    return [head.conv_seg, head.convs[0].bn, head.convs[0].conv] + unet_backward_order(unet) + \
+        embedder_linears(embedder)
+
+
+def unet_backward_order(unet):
+    """a UNet's ConvModules (bn, conv) in the order the backward pass finishes them: decoder blocks from the finest,
+    then encoder stages from the coarsest"""
     def cm(c):
         return [c.bn, c.conv]
-    order = [head.conv_seg] + cm(head.convs[0])
+    order = []
     for d in unet.decoder:
         for c in reversed(d.conv_block.convs):
             order += cm(c)
@@ -169,7 +177,7 @@ def backward_order(embedder, unet, head):
     for stage in reversed(unet.encoder):
         for c in reversed(stage[-1].convs):
             order += cm(c)
-    return order + embedder_linears(embedder)
+    return order
 
 
 def embedder_linears(emb):
