@@ -1,4 +1,5 @@
-"""Flat parameter store of the native trainers (``transformer_train``, ``vqgan_train``, ``segm_train``).
+"""Flat parameter store of the native trainers (``transformer_train``, ``vqgan_train``, ``segm_train``,
+``parsing_gen_train``, ``index_pred_train``).
 
 Parameters, gradients and Adam moments of an ordered list of modules live in four flat fp32 buffers and the
 ``nn.Parameter``s (and their ``.grad``) become views of them, so state_dict keys and shapes are unchanged and Adam is

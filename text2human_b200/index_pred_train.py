@@ -5,13 +5,14 @@ configs/index_pred_net.yml) on the H100 kernels.
   * ground truth from the frozen hierarchy (``feed_data``): ``feature_t`` = the top level's post-quant-conv feature
     (``top_encode_nhwc``, kept NHWC for the UNet) and, per latent position, the bottom quantizer's own-codebook index
     and texture id (bot_encoder -> bot_quant_conv -> the 2x2-patch ``vq_search``); ``bot_decoder_res`` is not run;
-  * the UNet guidance encoder (the ``index_pred_arch`` mirror) in training mode through the parsing generator's
-    layers (``BasicConvBlockL`` / ``UpConvBlockL``: conv -> BatchNorm2d on batch statistics -> ReLU); stage i > 0
-    reads MaxPool2d(2) of the previous stage, whose backward routes to each window's first maximum, added into that
-    stage's skip gradient; stage 0's input is the frozen feature, so its first conv computes no data gradient;
-  * the 18 heads of MultiHeadFCNHead: their 3x3 ConvModules run as ONE conv of 18*64 output channels (a
-    ``ConvStack`` in the parameter store), one BatchNorm over 1152 channels (the 18 BatchNorms' parameters and
-    running statistics are views of shared buffers), and the 18 Dropout2d draws as one head-major [B, 1152] factor;
+  * the UNet guidance encoder (the ``index_pred_arch`` mirror) in training mode through ``train_layers.UNetL``
+    (conv -> BatchNorm2d on batch statistics -> ReLU); stage i > 0 reads MaxPool2d(2) of the previous stage, whose
+    backward routes to each window's first maximum, added into that stage's skip gradient; stage 0's input is the
+    frozen feature, so its first conv computes no data gradient;
+  * the 18 heads of MultiHeadFCNHead: their 3x3 ConvModules run as ONE ``train_layers.ConvModuleL`` of 18*64
+    output channels (a ``ConvStack`` in the parameter store) with one BatchNorm over 1152 channels (the 18
+    BatchNorms' parameters and running statistics are views of shared buffers), and the 18 Dropout2d draws as one
+    head-major [B, 1152] factor;
   * loss: the sum over heads of CrossEntropyLoss(ignore_index=-1), i.e. each position's cross-entropy in its own
     texture's head (every other head ignores it), summed and divided by B*h*w, in one routed kernel
     (``routed_head_ce``) that scores each position with its own head only and writes the conv_seg gradients straight
@@ -19,19 +20,14 @@ configs/index_pred_net.yml) on the H100 kernels.
   * Adam (weight_decay 0) on one ``flat_params.ParamSpace``, gradient buckets all-reduced over the default process
     group while the backward pass runs, as in the other native trainers.
 """
-import math
-
 import torch
 import torch.nn as nn
 
-from . import conv_grad as G
 from . import ops
-from .dist import world_size
-from .flat_params import ConvStack, ParamSpace, drop_packed_caches, load_checkpoint, save_checkpoint
+from .flat_params import ConvStack, ParamSpace
 from .index_pred_arch import MultiHeadFCNHead, UNet
-from .parsing_gen_train import BasicConvBlockL, unet_backward_order, unet_decode_layers
+from .train_layers import ConvModuleL, SingleSpaceTrainer, UNetL
 from .vqgan_arch import conv1x1_nhwc
-from .vqgan_train import Layer
 
 NETS = ("guidance_encoder", "index_decoder")    # index_pred_net.pth (hierarchy_inference_model.py:310-323)
 IGNORE = -1                                     # the reference's ignore_index
@@ -51,67 +47,14 @@ class IndexPredNets(nn.Module):
             align_corners=opt['fc_align_corners'], num_head=18)
 
 
-class HeadConvsL(Layer):
-    """The heads' 3x3 ConvModules as one stacked ConvModule in training mode: conv (64 -> 18*64), BatchNorm2d over
-    the 1152 stacked channels (each channel's statistics are its own head's), ReLU, Dropout2d factor; ``fwd`` -> the
-    fp32 NHWC [B,h,w,18*64] that conv_seg reads, ``bwd`` -> the fp32 gradient of the input feature map."""
-
-    def __init__(self, tr, fcn, stack):
-        super().__init__(tr)
-        self.stack = stack
-        self.bns = tuple(seq[0].bn for seq in fcn.convs_list)
-        bn0 = self.bns[0]
-        assert all(bn.eps == bn0.eps and bn.momentum == bn0.momentum and bn.track_running_stats for bn in self.bns)
-        self.eps, self.momentum = bn0.eps, bn0.momentum
-        sp = tr.space
-        self.gamma, self.dgamma = sp.joint([bn.weight for bn in self.bns])
-        self.beta, self.dbeta = sp.joint([bn.bias for bn in self.bns])
-        # running statistics and step counters: views into one buffer each, so that one bn_update_running launch
-        # (and one increment) serves the 18 BatchNorms; state_dict / load_state_dict see the same tensors as before
-        C = fcn.channels
-        with torch.no_grad():
-            self.rmean = torch.cat([bn.running_mean.float() for bn in self.bns]).contiguous()
-            self.rvar = torch.cat([bn.running_var.float() for bn in self.bns]).contiguous()
-            self.nbt = torch.stack([bn.num_batches_tracked for bn in self.bns]).contiguous()
-        for k, bn in enumerate(self.bns):
-            bn.running_mean = self.rmean[k * C:(k + 1) * C]
-            bn.running_var = self.rvar[k * C:(k + 1) * C]
-            bn.num_batches_tracked = self.nbt[k]
-
-    def fwd(self, a, drop):
-        """a planes [T,B,h,w,Cin] -> ReLU(BN(conv(a))) [* drop[image, channel]] fp32 NHWC"""
-        _, N, H, W, _ = a.shape
-        cp = self.cp(self.stack)
-        pre = G.forward("k3", a, cp.wn, None, n=N, in_hw=(H, W))
-        st = ops.norm_stats(pre, cp.co, n=1)
-        ops.bn_update_running(st, self.rmean, self.rvar, N * H * W, self.momentum)
-        self.nbt += 1
-        y, _ = ops.norm_apply_ex(pre, st, self.gamma, self.beta, act="relu", groups=cp.co, eps=self.eps, n=1,
-                                 drop=drop, want_f32=True)
-        self.saved.append((a, pre, st, drop))
-        return y
-
-    def bwd(self, dy):
-        a, pre, st, drop = self.saved.pop()
-        N, H, W, _ = pre.shape
-        cp = self.cp(self.stack)
-        _, dpre = ops.norm_bwd(pre, st, self.gamma, self.beta, dy, act="relu", groups=cp.co, eps=self.eps,
-                               dgamma=self.dgamma, dbeta=self.dbeta, want_planes=True, want_dx=False, n=1,
-                               dy_scale=drop)
-        for bn in self.bns:
-            self.done(bn)
-        G.wgrad("k3", dpre, a, cp.gw, n=N)
-        self.done(self.stack)
-        return G.dgrad("k3", dpre, cp.wt, n=N, in_hw=(H, W))
-
-
-class IndexPredTrainer:
+class IndexPredTrainer(SingleSpaceTrainer):
     """Owns the two mirror nets (``unet`` index_pred_arch.UNet, ``fcn`` MultiHeadFCNHead) and, for ``feed_data``,
     the frozen ``hierarchy`` (a pipeline.HierarchyVQSpatialTextureAwareModel loaded from vqvae_top.pth /
     vqvae_bottom.pth; may be None when the caller supplies the ground truth).  ``optimize_parameters`` is one
     reference training step; ``lr`` may be changed between steps.  The nets stay in eval mode: their inference path
     (``UNet.forward_nhwc``, ``MultiHeadFCNHead.forward_logits``, ``bot_index_prediction``) sees the trained
-    parameters and running statistics after every Adam step and every load."""
+    parameters and running statistics after every Adam step and every load.  Checkpoints have the reference layout
+    (hierarchy_inference_model.py:310-323) plus the optimiser state."""
 
     def __init__(self, unet, fcn, hierarchy=None, lr=1e-4, weight_decay=0.0, betas=(0.9, 0.999), eps=1e-8,
                  bucket_bytes=48 << 20):
@@ -127,32 +70,20 @@ class IndexPredTrainer:
         self.stack = ConvStack(seq[0].conv for seq in fcn.convs_list)
         self.segs = tuple(fcn.conv_seg_head_list)
         bns = tuple(seq[0].bn for seq in fcn.convs_list)
-        self.space = ParamSpace([self.segs, bns, self.stack] + unet_backward_order(unet), self.device, bucket_bytes)
+        self.unet_l = UNetL(self, unet, need_dx=False)
+        self.space = ParamSpace([self.segs, bns, self.stack] + self.unet_l.order(), self.device, bucket_bytes)
         G_, K, C = self.n_head, self.n_classes, self.channels
         w, gw = self.space.joint([c.weight for c in self.segs], C)
         b, gb = self.space.joint([c.bias for c in self.segs])
         self.w_seg, self.gw_seg = w.view(G_, K, C), gw.view(G_, K, C)
         self.b_seg, self.gb_seg = b.view(G_, K), gb.view(G_, K)
-        self.stages = [BasicConvBlockL(self, s[-1], need_dx=i > 0) for i, s in enumerate(unet.encoder)]
-        self.dec = unet_decode_layers(self, unet.decoder)
-        self.head = HeadConvsL(self, fcn, self.stack)
+        self.head = ConvModuleL(self, self.stack, bns, "k3", "relu")
         self._gt = None
         self._out = None
         self._sync_from_rank0()
 
-    # ---- plumbing used by the layers
-    def space_of(self, mod):
-        return self.space
-
-    def space_of_param(self, p):
-        return self.space
-
     def _nets(self):
         return dict(guidance_encoder=self.unet, index_decoder=self.fcn)
-
-    def _sync_from_rank0(self):
-        self.space.sync_from_rank0()
-        drop_packed_caches(*self._nets().values())
 
     def draw_dropout_mask(self, B, generator=None):
         """the 18 nn.Dropout2d draws of one step, in head order: [num_head, B, channels] Bernoulli(1-p)"""
@@ -253,23 +184,12 @@ class IndexPredTrainer:
         x, own, tex = self._batch(data, feature_t, targets)
         B, h, w, _ = x.shape
         M = B * h * w
-        # static loss scale (a power of two, undone inside Adam): d loss / d logit ~ 1/M is below fp16 resolution
-        S = self.loss_scale = 2.0 ** math.floor(math.log2(M))
+        S = self._begin_step(M)
         sp = self.space
-        sp.flat_g.zero_()
-        sp.prepare(ops.get_terms())
         # ---- UNet encoder / decoder (unet_arch.py:460-471)
-        a = ops.f32_to_planes(x)
-        enc = []
-        for i, stage in enumerate(self.stages):
-            if i > 0:
-                a = ops.f32_to_planes(enc[-1], ops.CVT_MAXPOOL2)
-            enc.append(stage.fwd(a))
-        x = enc[-1]
-        for i in reversed(range(len(self.dec))):
-            x = self.dec[i].fwd(enc[i], x)
+        x = self.unet_l.fwd(x)
         # ---- heads and the routed loss
-        y = self.head.fwd(ops.f32_to_planes(x), drop)
+        y = self.head.fwd(ops.f32_to_planes(x), out="f32", drop=drop)
         loss = torch.zeros(1, dtype=torch.float64, device=self.device)
         sp.arm(True)
         dy = ops.routed_head_ce(y.view(M, -1), tex, own, self.w_seg, self.b_seg, loss, self.gw_seg, self.gb_seg,
@@ -280,15 +200,7 @@ class IndexPredTrainer:
         # ---- backward
         d = self.head.bwd(dy.view(B, h, w, -1))
         del dy
-        d_skip = [None] * len(self.dec)
-        for i in range(len(self.dec)):
-            d_skip[i], d = self.dec[i].bwd(d)
-        for i in reversed(range(len(self.stages))):
-            da = self.stages[i].bwd(d)
-            if i > 0:
-                d = d_skip[i - 1]
-                ops.maxpool2_bcast_bwd(da, enc[i - 1].shape[-1], 0, x=enc[i - 1], dx=d, pool=True,
-                                       in_hw=enc[i - 1].shape[1:3], accumulate=True)
+        self.unet_l.bwd(d)
         sp.release()
         self._out = dict(loss=loss, npix=M)
         return self._out
@@ -297,11 +209,6 @@ class IndexPredTrainer:
         """the reference's log_dict (hierarchy_inference_model.py:245); one device->host read"""
         o = self._out
         return dict(loss_total=float(o["loss"][0]) / o["npix"])
-
-    def adam_step(self):
-        self.space.wait()
-        self.space.adam(self.lr, self.betas, self.eps, 1.0 / (world_size() * self.loss_scale))
-        drop_packed_caches(*self._nets().values())
 
     def optimize_parameters(self, data=None, dropout_mask=None, *, feature_t=None, targets=None):
         self.training_step(data, dropout_mask, feature_t=feature_t, targets=targets)
@@ -327,13 +234,3 @@ class IndexPredTrainer:
             acc += float(((pred == own.reshape(-1)) & live).sum()) / (h * w)
             num += B
         return acc / num
-
-    # ---- checkpoint / resume: the reference layout (hierarchy_inference_model.py:310-323) plus the optimiser state
-    def save(self, path):
-        save_checkpoint(path, self._nets(), self.space.state())
-
-    def load(self, path):
-        opt = load_checkpoint(path, self._nets(), self.device)
-        if opt is not None:
-            self.space.load_state(opt)
-        self._sync_from_rank0()

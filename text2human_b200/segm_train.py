@@ -14,14 +14,14 @@ reference's ``training_step`` + ``loss.backward()`` + ``optimizer.step()``:
   * loss: ``bce_logits`` reads the decoder's NHWC logits and the ids once and writes the output gradient as the
     fp16 planes conv_out's gradients read, plus conv_out's bias gradient (DESIGN §4.4);
   * parameters, gradients and Adam moments in one ``flat_params.ParamSpace``, whose gradient buckets are all-reduced
-    over the default process group while the backward pass runs, as in ``VQGANTrainer``.
+    over the default process group while the backward pass runs, as in ``VQGANTrainer``; the loss scale, Adam step
+    and checkpoints are ``train_layers.SingleSpaceTrainer``'s.
 
 The drop-in path for the same step (the reference's own ``optimize_parameters`` on the arch mirrors) goes through
 the autograd nodes of ``vqgan_autograd``.
 """
 import contextlib
 import io
-import math
 
 import torch
 import torch.nn as nn
@@ -29,8 +29,8 @@ import torch.nn as nn
 from . import conv_grad as G
 from . import ops
 from . import vqgan_train as VT
-from .dist import world_size
-from .flat_params import ParamSpace, drop_packed_caches, load_checkpoint, save_checkpoint
+from .flat_params import ParamSpace
+from .train_layers import SingleSpaceTrainer
 from .vqgan_train import NETS
 from .vqgan_arch import Decoder, Encoder, VectorQuantizer
 
@@ -69,11 +69,12 @@ class ConvInPlanesL(VT.ConvInImageL):
         return VT.Act(y, st)
 
 
-class SegmTokenizerTrainer:
+class SegmTokenizerTrainer(SingleSpaceTrainer):
     """Owns a model with ``encoder``, ``decoder``, ``quantize`` (VectorQuantizer), ``quant_conv``,
     ``post_quant_conv`` (e.g. ``SegmTokenizerModel``); ``optimize_parameters(data)`` is one reference training step
     on ``data['segm']``, the parsing map of MaskDataset (class ids [B,H,W] or [B,1,H,W]).  ``lr`` may be changed
-    between steps (the reference's step decay runs on the host)."""
+    between steps (the reference's step decay runs on the host).  Checkpoints have the reference layout (what
+    load_pretrained_segm_token reads, sample_model.py:154-166) plus the optimiser state."""
 
     def __init__(self, model, lr=4.5e-5, betas=(0.5, 0.9), eps=1e-8, bucket_bytes=48 << 20):
         self.model = model
@@ -96,16 +97,8 @@ class SegmTokenizerTrainer:
         self._out = None
         self._sync_from_rank0()
 
-    # ---- plumbing used by the layers
-    def space_of(self, mod):
-        return self.space
-
-    def space_of_param(self, p):
-        return self.space
-
-    def _sync_from_rank0(self):
-        self.space.sync_from_rank0()
-        drop_packed_caches(self.model)
+    def _nets(self):
+        return {k: getattr(self.model, k) for k in NETS}
 
     # ---- one step
     def training_step(self, data):
@@ -119,11 +112,8 @@ class SegmTokenizerTrainer:
         B, _, H, W = segm.shape
         C = self.n_classes
         nel = B * C * H * W
-        # static loss scale (a power of two, undone inside Adam): d bce / d logit ~ 1/nel is below fp16 resolution
-        S = self.loss_scale = 2.0 ** math.floor(math.log2(nel))
+        S = self._begin_step(nel)
         sp, dev = self.space, self.device
-        sp.flat_g.zero_()
-        sp.prepare(ops.get_terms())
         h = self.enc_out.fwd(self.enc_body.fwd(self.enc_in.fwd(ops.onehot_to_planes(segm, C))))
         z = self.qconv.fwd(h)
         del h
@@ -157,25 +147,6 @@ class SegmTokenizerTrainer:
         quant = (1.0 + self.beta) * float(o["sqerr"][0]) / o["z_numel"]
         return dict(total_loss=bce + quant, bce_loss=bce, quant_loss=quant)
 
-    def adam_step(self):
-        self.space.wait()
-        self.space.adam(self.lr, self.betas, self.eps, 1.0 / (world_size() * self.loss_scale))
-        drop_packed_caches(self.model)
-
     def optimize_parameters(self, data):
         self.training_step(data)
         self.adam_step()
-
-    # ---- checkpoint / resume: the reference layout (what load_pretrained_segm_token reads, sample_model.py:154-166)
-    # plus the optimiser state
-    def _nets(self):
-        return {k: getattr(self.model, k) for k in NETS}
-
-    def save(self, path):
-        save_checkpoint(path, self._nets(), self.space.state())
-
-    def load(self, path):
-        opt = load_checkpoint(path, self._nets(), self.device)
-        if opt is not None:
-            self.space.load_state(opt)
-        self._sync_from_rank0()

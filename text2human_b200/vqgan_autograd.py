@@ -141,6 +141,8 @@ def _all_layers(objs):
     for o in objs:
         if isinstance(o, VT.Seq):
             out += o.layers
+        elif isinstance(o, VT.DiscNet):
+            out += [o] + o.mid
         elif o is not None:
             out.append(o)
     return out

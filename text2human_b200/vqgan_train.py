@@ -30,6 +30,7 @@ from . import ops
 from .dist import world_size
 from .flat_params import ParamSpace, drop_packed_caches, load_checkpoint, save_checkpoint
 from .ops import CVT_PLAIN, CVT_S2D, CVT_UP2X
+from .train_layers import ConvModuleL, Grad, Layer
 from .vqgan_arch import AttnBlock, Decoder, Discriminator, Downsample, Encoder, ResnetBlock, Upsample
 
 NETS = ("encoder", "decoder", "quantize", "quant_conv", "post_quant_conv")    # the generator's nets, as checkpointed
@@ -47,48 +48,8 @@ class Act:
         self.x, self.stats = x, stats
 
 
-class Grad:
-    """gradient wrt an activation: fp32 NHWC + (optionally) its fp16 planes and its column sums (what the producing
-    norm-backward kernel accumulated on the side: the bias gradient of the conv this activation came out of)"""
-    __slots__ = ("g", "p", "colsum")
-
-    def __init__(self, g, p=None, colsum=None):
-        self.g, self.p, self.colsum = g, p, colsum
-
-    def planes(self):
-        if self.p is None:
-            self.p = ops.f32_to_planes(self.g, CVT_PLAIN)
-        return self.p
-
-
 def _stats(act, groups=32):
     return act.stats if act.stats is not None else ops.norm_stats(act.x, groups)
-
-
-class Layer:
-    def __init__(self, tr):
-        self.tr = tr
-        self.saved = []
-
-    def cp(self, mod):
-        return self.tr.space_of(mod).convs[mod]
-
-    def gof(self, p):
-        return self.tr.space_of_param(p).g(p)
-
-    def done(self, mod):
-        self.tr.space_of(mod).done(mod)
-
-    def bias_grad(self, cp, g):
-        """cp.gb += column sums of the output gradient ``g`` (a Grad, or a bare fp32 NHWC tensor)"""
-        if cp.gb is None:
-            return
-        t = g.g if isinstance(g, Grad) else g
-        Cc = t.shape[-1]
-        if isinstance(g, Grad) and g.colsum is not None:
-            ops.add_inplace(cp.gb[:Cc], g.colsum)
-        else:
-            ops.colsum_(cp.gb[:Cc], t.reshape(-1, Cc))
 
 
 class ConvL(Layer):
@@ -502,52 +463,33 @@ class DiscNet(Layer):
     def __init__(self, tr, disc):
         super().__init__(tr)
         mods = list(disc.main)
-        self.first = mods[0]
-        self.mid = []          # (conv, bn, kind)
-        i = 2
-        while i + 2 < len(mods):
-            conv, bn = mods[i], mods[i + 1]
-            self.mid.append((conv, bn, "k4s2" if conv.stride[0] == 2 else "k4s1"))
-            i += 3
-        self.last = mods[-1]
+        self.first, self.last = mods[0], mods[-1]
+        self.mid = [ConvModuleL(tr, conv, (bn,), "k4s2" if conv.stride[0] == 2 else "k4s1", "lrelu")
+                    for conv, bn in zip(mods[2:-1:3], mods[3:-1:3])]
 
     def order(self):
-        out = [self.last]
-        for conv, bn, _ in reversed(self.mid):
-            out += [bn, conv]
-        return out + [self.first]
+        return [self.last] + [m for cm in reversed(self.mid) for m in (cm.bns[0], cm.conv)] + [self.first]
 
     def fwd(self, x_nchw):
         """fp32 NCHW image batch -> logits fp32 [N,h,w,1]"""
         N, _, H, W = x_nchw.shape
-        rec = []
         c0 = self.cp(self.first)
         a0 = ops.planes_s2d(ops.nchw_to_planes(x_nchw))
         y0 = G.forward("k4s2", a0, c0.wn, c0.b, n=N, in_hw=(H, W), planes_out=True, act=ops.ACT_LRELU)
-        rec.append((a0, y0, H, W))
-        h, hh, ww = y0, H // 2, W // 2
-        for conv, bn, kind in self.mid:
-            cp = self.cp(conv)
-            a = ops.planes_s2d(h) if kind == "k4s2" else h
-            pre = G.forward(kind, a, cp.wn, None, n=N, in_hw=(hh, ww))
-            st = ops.norm_stats(pre, pre.shape[-1], n=1)
-            Cc = pre.shape[-1]
-            ops.bn_update_running(st, bn.running_mean, bn.running_var, pre.numel() // Cc, bn.momentum)
-            bn.num_batches_tracked += 1
-            h = ops.norm_apply(pre, st, bn.weight.detach(), bn.bias.detach(), act="lrelu", groups=Cc, eps=bn.eps, n=1)
-            rec.append((a, pre, st, hh, ww))
-            hh, ww = G.out_hw(kind, hh, ww)
+        h = y0
+        for m in self.mid:
+            self.cp(m.conv)     # a StandaloneSpace packs a conv's weights at its first lookup, ahead of the operand
+            h = m.fwd(ops.planes_s2d(h) if m.kind == "k4s2" else h)
         cl = self.cp(self.last)
-        logits = G.forward("k4s1", h, cl.wn[:, :, :1], cl.b[:1], n=N, in_hw=(hh, ww))
-        rec.append((h, hh, ww, N))
-        self.saved.append(rec)
+        logits = G.forward("k4s1", h, cl.wn[:, :, :1], cl.b[:1], n=N, in_hw=h.shape[2:4])
+        self.saved.append((a0, y0, H, W, h))
         return logits
 
     def bwd(self, dlogits, want_params, want_input, dx_out=None):
         """dlogits fp32 [N,h,w,1]; parameter gradients are accumulated when ``want_params``; with ``want_input`` the
         image gradient is written to ``dx_out`` fp32 NCHW [N,3,H,W]"""
-        rec = self.saved.pop()
-        h, hh, ww, N = rec.pop()
+        a0, y0, H, W, h = self.saved.pop()
+        _, N, hh, ww, _ = h.shape
         cl = self.cp(self.last)
         ho, wo = dlogits.shape[1:3]
         dlp = ops.nchw_to_planes(dlogits.view(N, 1, ho, wo))                 # [T,N,ho,wo,8]
@@ -556,20 +498,8 @@ class DiscNet(Layer):
             G.wgrad("k4s1", dlp, h, cl.gw, n=N)
             self.done(self.last)
         g = G.dgrad("k4s1", dlp, cl.wt, n=N, in_hw=(hh, ww))
-        for conv, bn, kind in reversed(self.mid):
-            a, pre, st, hh, ww = rec.pop()
-            cp = self.cp(conv)
-            Cc = pre.shape[-1]
-            dpre, dprep = ops.norm_bwd(pre, st, bn.weight.detach(), bn.bias.detach(), g, act="lrelu", groups=Cc,
-                                       eps=bn.eps, dgamma=self.gof(bn.weight) if want_params else None,
-                                       dbeta=self.gof(bn.bias) if want_params else None, want_planes=True, n=1,
-                                       want_dx=False)
-            if want_params:
-                self.done(bn)
-                G.wgrad(kind, dprep, a, cp.gw, n=N)
-                self.done(conv)
-            g = G.dgrad(kind, dprep, cp.wt, n=N, in_hw=(hh, ww))
-        a0, y0, H, W = rec.pop()
+        for m in reversed(self.mid):
+            g = m.bwd(g, want_params=want_params)
         c0 = self.cp(self.first)
         dpre, dprep = ops.lrelu_bwd(y0, g)
         if want_params:
