@@ -285,6 +285,19 @@ int t2h_vq_gather(const float* codebook, const int64_t* idx, const int32_t* book
                   int b, int hz, int wz, int cz, int ps, int n_books, int n_e,
                   float* zq_nhwc, float* zq_nchw, t2h_stream_t stream);
 
+/* Backward of the texture quantizers over ps x ps patches
+ * (VectorQuantizerSpatialTextureAware.forward :438-454; ps == 1 is VectorQuantizerTexture): with the row / patch
+ * address map of t2h_vq_search,
+ *   dz[NHWC] = dzq + coef_z * (z - e)               (e = 0 for rows whose book_id or idx selects no code)
+ *   dcodebook[book][idx] += coef_e * (e - z_patch)  summed over the rows of each code in ascending row order
+ * The codebook gradient is a stable sort of the rows by (book, code) and a per-code reduction: no floating-point
+ * atomics, reruns are bitwise equal.  dzq may be NULL (zero).  order: int32 [rows], off: int32
+ * [n_books*n_e + 2] workspace.  n_books*n_e <= 12287. */
+int t2h_vq_bwd_patch(const float* z, const float* codebook, const int64_t* idx, const int32_t* book_id,
+                     const float* dzq, float* dz, float* dcodebook, int32_t* order, int32_t* off,
+                     int b, int hz, int wz, int cz, int ps, int n_books, int n_e, float coef_z,
+                     float coef_e, t2h_stream_t stream);
+
 /* segmentation ids [B,1,H,W] (float) -> one-hot fp16 planes NHWC [terms][B][H][W][c_pad]: the input of the
  * segm tokeniser's Encoder; replaces F.one_hot(...).permute(0,3,1,2).float() (sample_model.py:331-335) */
 int t2h_onehot_to_planes(const float* ids, void* out, int b, int h, int w, int n_classes, int c_pad, int terms,

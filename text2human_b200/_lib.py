@@ -86,6 +86,7 @@ SIGNATURES = {
                            _P, _L, _P]),
     "t2h_vq_workspace_bytes": (_L, [_L, _I, _I]),
     "t2h_vq_gather": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
+    "t2h_vq_bwd_patch": (_I, [_P] * 9 + [_I] * 7 + [_F, _F, _P]),
     "t2h_texture_mask": (_I, [_P, _P, _P, _I, _P, _I, _L, _P]),
     "t2h_u8_to_planes": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _F, _F, _I, _P]),
     "t2h_mask_to_ids": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),

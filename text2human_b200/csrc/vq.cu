@@ -323,6 +323,123 @@ __global__ void vq_gather_kernel(const float* __restrict__ cb, const long long* 
   }
 }
 
+// ---- patch quantizer backward (VectorQuantizerSpatialTextureAware.forward :438-454): zq_st = z + (zq - z).detach(),
+// loss = mean((zq.detach()-z)^2) + beta*mean((zq - z.detach())^2) over the folded patches:
+//   dz = dzq + coef_z * (z - e)                 (e = 0 for rows no codebook selects)
+//   dE[book][code] += coef_e * (e - z_patch)    summed over the rows that chose the code, in ascending row order
+// The codebook gradient uses no floating-point atomics: rows are sorted by (book, code) with a stable counting sort,
+// then one warp reduces each code's segment, so reruns are bitwise equal.
+constexpr int kVqSortThreads = 1024;
+
+__device__ __forceinline__ int vq_code_key(const long long* __restrict__ idx, const int* __restrict__ book, int r,
+                                           int n_books, int n_e) {
+  const int k = book ? book[r] : 0;
+  const long long id = idx[r];
+  return (k >= 0 && k < n_books && id >= 0 && id < n_e) ? k * n_e + (int)id : n_books * n_e;
+}
+
+// One CTA.  off[key] = first slot of key (n_books*n_e keys + the bin of rows without a code), off[nb] = rows;
+// order[slot] = row, rows in ascending order inside each key.
+__global__ void __launch_bounds__(kVqSortThreads) vq_patch_sort_kernel(const long long* __restrict__ idx,
+                                                                       const int* __restrict__ book, int rows,
+                                                                       int n_books, int n_e, int* __restrict__ order,
+                                                                       int* __restrict__ off) {
+  extern __shared__ int cur[];  // [nb]: counts, then write cursors
+  __shared__ int wsum[kVqSortThreads / 32];
+  const int nb = n_books * n_e + 1;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int i = tid; i < nb; i += kVqSortThreads) cur[i] = 0;
+  __syncthreads();
+  for (int r = tid; r < rows; r += kVqSortThreads) atomicAdd(&cur[vq_code_key(idx, book, r, n_books, n_e)], 1);
+  __syncthreads();
+  // exclusive scan: thread t owns the contiguous bins [lo, hi)
+  const int per = (nb + kVqSortThreads - 1) / kVqSortThreads;
+  const int lo = min(nb, tid * per), hi = min(nb, lo + per);
+  int s = 0;
+  for (int i = lo; i < hi; ++i) s += cur[i];
+  int incl = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  if (lane == 31) wsum[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    int w = wsum[lane], wi = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, wi, o);
+      if (lane >= o) wi += v;
+    }
+    wsum[lane] = wi - w;
+  }
+  __syncthreads();
+  int base = wsum[warp] + incl - s;
+  for (int i = lo; i < hi; ++i) {
+    const int c = cur[i];
+    cur[i] = off[i] = base;
+    base += c;
+  }
+  if (tid == 0) off[nb] = rows;
+  __syncthreads();
+  // stable scatter by one warp, 32 rows at a time: a row's rank among the equal keys of its 32 comes from
+  // __match_any_sync, the lowest such lane advances the key's cursor
+  if (warp != 0) return;
+  for (int t0 = 0; t0 < rows; t0 += 32) {
+    const int r = t0 + lane;
+    const int k = r < rows ? vq_code_key(idx, book, r, n_books, n_e) : -1;
+    const unsigned same = __match_any_sync(0xffffffffu, k);
+    const int rank = __popc(same & ((1u << lane) - 1u));
+    const int c = r < rows ? cur[k] : 0;
+    __syncwarp();
+    if (r < rows) {
+      order[c + rank] = r;
+      if (rank == 0) cur[k] = c + __popc(same);
+    }
+    __syncwarp();
+  }
+}
+
+// dz over the NHWC elements of z (coalesced); the patch row and in-patch index come from the F.unfold order
+__global__ void vq_patch_dz_kernel(const float* __restrict__ z, const float* __restrict__ cb,
+                                   const long long* __restrict__ idx, const int* __restrict__ book,
+                                   const float* __restrict__ dzq, VqShape s, float coef_z, float* __restrict__ dz) {
+  const long long total = (long long)s.B * s.Hz * s.Wz * s.Cz;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % s.Cz);
+    const long long pix = i / s.Cz;
+    const int x = (int)(pix % s.Wz);
+    const int y = (int)((pix / s.Wz) % s.Hz);
+    const int b = (int)(pix / ((long long)s.Wz * s.Hz));
+    const int row = (b * s.Hp + y / s.ps) * s.Wp + x / s.ps;
+    const int d = c * s.ps * s.ps + (y % s.ps) * s.ps + x % s.ps;
+    const int key = vq_code_key(idx, book, row, s.n_books, s.n_e);
+    const float ev = key < s.n_books * s.n_e ? cb[(long long)key * s.D + d] : 0.f;
+    dz[i] = (dzq ? dzq[i] : 0.f) + coef_z * (z[i] - ev);
+  }
+}
+
+// one warp per code: dE[code][d] += coef_e * (e[d] - z_row[d]) for the code's rows in slot (= row) order
+__global__ void __launch_bounds__(256) vq_patch_de_kernel(const float* __restrict__ z, const float* __restrict__ cb,
+                                                          const int* __restrict__ order, const int* __restrict__ off,
+                                                          VqShape s, float coef_e, float* __restrict__ dcb) {
+  const int code = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (code >= s.n_books * s.n_e) return;
+  const int beg = off[code], end = off[code + 1];
+  if (beg == end) return;
+  const float* e = cb + (long long)code * s.D;
+  float* de = dcb + (long long)code * s.D;
+  for (int d = lane; d < s.D; d += 32) {
+    const float ev = e[d];
+    float acc = de[d];
+    for (int i = beg; i < end; ++i)
+      acc = __fadd_rn(acc, __fmul_rn(coef_e, __fsub_rn(ev, z[z_offset(s, order[i], d)])));
+    de[d] = acc;
+  }
+}
+
 static int make_shape(VqShape* s, int b, int hz, int wz, int cz, int ps, int n_books, int n_e) {
   T2H_CHECK_ARG(b > 0 && hz > 0 && wz > 0 && cz > 0, "vq: bad z shape");
   T2H_CHECK_ARG(ps == 1 || ps == 2, "vq: patch size %d unsupported", ps);
@@ -398,6 +515,30 @@ int t2h_vq_gather(const float* codebook, const int64_t* idx, const int32_t* book
   if (g > num_sms() * 16LL) g = num_sms() * 16LL;
   vq_gather_kernel<<<(int)g, 256, 0, as_stream(stream)>>>(codebook, reinterpret_cast<const long long*>(idx),
                                                          book_id, s, zq_nhwc, zq_nchw);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_vq_bwd_patch(const float* z, const float* codebook, const int64_t* idx, const int32_t* book_id,
+                     const float* dzq, float* dz, float* dcodebook, int32_t* order, int32_t* off, int b, int hz, int wz,
+                     int cz, int ps, int n_books, int n_e, float coef_z, float coef_e, t2h_stream_t stream) {
+  T2H_CHECK_ARG(z && codebook && idx && dz && dcodebook && order && off, "vq_bwd_patch: null pointer");
+  VqShape s;
+  int rc = make_shape(&s, b, hz, wz, cz, ps, n_books, n_e);
+  if (rc) return rc;
+  const size_t smem = (size_t)(n_books * n_e + 1) * sizeof(int);
+  T2H_CHECK_ARG(smem <= 48 * 1024, "vq_bwd_patch: n_books*n_e=%d codes too many for the sort", n_books * n_e);
+  cudaStream_t st = as_stream(stream);
+  const long long* id = reinterpret_cast<const long long*>(idx);
+  vq_patch_sort_kernel<<<1, kVqSortThreads, smem, st>>>(id, book_id, s.rows, n_books, n_e, order, off);
+  T2H_LAUNCH_OK();
+  const long long total = (long long)b * hz * wz * cz;
+  long long g = ceil_div64(total, 256);
+  if (g > num_sms() * 16LL) g = num_sms() * 16LL;
+  vq_patch_dz_kernel<<<(int)g, 256, 0, st>>>(z, codebook, id, book_id, dzq, s, coef_z, dz);
+  T2H_LAUNCH_OK();
+  vq_patch_de_kernel<<<(unsigned)ceil_div64((long long)n_books * n_e, 8), 256, 0, st>>>(z, codebook, order, off, s,
+                                                                                         coef_e, dcodebook);
   T2H_LAUNCH_OK();
   return T2H_OK;
 }

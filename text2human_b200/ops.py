@@ -1218,6 +1218,27 @@ def vq_bwd(z, codebook, idx, book_id, dzq, dcodebook, coef_z, coef_e):
     return dz
 
 
+def vq_bwd_patch(z, codebook, idx, book_id, dzq, dcodebook, coef_z, coef_e, ps=2):
+    """Quantizer backward over ps x ps patches (see t2h_vq_bwd_patch): z / dzq fp32 NHWC [B,Hz,Wz,Cz], codebook
+    fp32 [n_books, n_e, Cz*ps*ps], idx int64 [B,Hz/ps,Wz/ps], book_id int32 of the same shape (or None: book 0).
+    dcodebook[book, idx] += coef_e (e - z_patch) in a fixed order; -> dz = dzq + coef_z (z - e), NHWC."""
+    _need_cuda(z, codebook, idx)
+    B, Hz, Wz, Cz = z.shape
+    n_books, n_e, D = codebook.shape
+    assert D == Cz * ps * ps and z.is_contiguous() and codebook.is_contiguous() and dcodebook.is_contiguous()
+    assert dcodebook.shape == codebook.shape and (dzq is None or (dzq.shape == z.shape and dzq.is_contiguous()))
+    rows = B * (Hz // ps) * (Wz // ps)
+    assert idx.numel() == rows and (book_id is None or book_id.numel() == rows)
+    dz = torch.empty_like(z)
+    order = torch.empty((rows,), dtype=torch.int32, device=z.device)
+    off = torch.empty((n_books * n_e + 2,), dtype=torch.int32, device=z.device)
+    _count(3)
+    _lib.check(_lib.load().t2h_vq_bwd_patch(_ptr(z), _ptr(codebook), _ptr(idx.contiguous()), _ptr(book_id), _ptr(dzq),
+                                            _ptr(dz), _ptr(dcodebook), _ptr(order), _ptr(off), B, Hz, Wz, Cz, ps,
+                                            n_books, n_e, coef_z, coef_e, _stream()))
+    return dz
+
+
 def l1_loss(x, xrec, sum_out, gscale=0.0, want_grad=True):
     """sum_out[0] += sum|x - xrec|; -> grad = gscale*sign(xrec - x) (or None)"""
     _need_cuda(x, xrec)

@@ -398,13 +398,20 @@ def encoder_layers(tr, enc):
                 body.append(AttnL(tr, lvl.attn[i_block]))
         if i_level != enc.num_resolutions - 1:
             body.append(ConvL(tr, lvl.downsample.conv, "down", pre="s2d"))
-    body += [ResL(tr, enc.mid.block_1), AttnL(tr, enc.mid.attn_1), ResL(tr, enc.mid.block_2)]
+    body += mid_layers(tr, enc.mid)
     return ConvInImageL(tr, enc.conv_in), Seq(body), NormConvOutL(tr, enc.norm_out, enc.conv_out, nchw=False)
 
 
-def decoder_layers(tr, dec):
-    body = [ResL(tr, dec.mid.block_1), AttnL(tr, dec.mid.attn_1), ResL(tr, dec.mid.block_2)]
-    for i_level in reversed(range(dec.num_resolutions)):
+def mid_layers(tr, mid):
+    """the middle block (ResnetBlock, AttnBlock, ResnetBlock) of an Encoder, Decoder or DecoderRes"""
+    return [ResL(tr, mid.block_1), AttnL(tr, mid.attn_1), ResL(tr, mid.block_2)]
+
+
+def decoder_up_layers(tr, dec, top_level):
+    """the decoder's levels ``top_level`` down to 0 (blocks, attention, the upsample of every level but 0), in
+    forward order"""
+    body = []
+    for i_level in reversed(range(top_level + 1)):
         lvl = dec.up[i_level]
         for i_block in range(dec.num_res_blocks + 1):
             body.append(ResL(tr, lvl.block[i_block]))
@@ -412,44 +419,69 @@ def decoder_layers(tr, dec):
                 body.append(AttnL(tr, lvl.attn[i_block]))
         if i_level != 0:
             body.append(ConvL(tr, lvl.upsample.conv, "k3", pre="up2x"))
+    return body
+
+
+def decoder_layers(tr, dec):
+    body = mid_layers(tr, dec.mid) + decoder_up_layers(tr, dec, dec.num_resolutions - 1)
     return ConvL(tr, dec.conv_in, "k3"), Seq(body), NormConvOutL(tr, dec.norm_out, dec.conv_out, nchw=True)
 
 
-def backward_order(model, disc=None):
-    """leaf modules of the generator in the order the backward pass finishes their gradients"""
-    def res(b):
-        out = [b.conv2, b.norm2, b.conv1]
-        if b.in_channels != b.out_channels:
-            out.append(b.nin_shortcut)
-        return out + [b.norm1]
+def _res_order(b):
+    out = [b.conv2, b.norm2, b.conv1]
+    if b.in_channels != b.out_channels:
+        out.append(b.nin_shortcut)
+    return out + [b.norm1]
 
-    def attn(a):
-        return [a.proj_out, (a.q, a.k, a.v), a.norm]
-    dec, enc = model.decoder, model.encoder
-    order = [dec.conv_out, dec.norm_out]
-    for i_level in range(dec.num_resolutions):
+
+def _attn_order(a):
+    return [a.proj_out, (a.q, a.k, a.v), a.norm]
+
+
+def mid_order(mid):
+    """the middle block's leaf modules in backward-completion order"""
+    return _res_order(mid.block_2) + _attn_order(mid.attn_1) + _res_order(mid.block_1)
+
+
+def decoder_up_order(dec, top_level):
+    """leaf modules of the decoder's levels 0..``top_level`` in backward-completion order (norm_out / conv_out
+    excluded)"""
+    order = []
+    for i_level in range(top_level + 1):
         lvl = dec.up[i_level]
         if i_level != 0:
             order.append(lvl.upsample.conv)
         for i_block in reversed(range(dec.num_res_blocks + 1)):
             if len(lvl.attn) > 0:
-                order += attn(lvl.attn[i_block])
-            order += res(lvl.block[i_block])
-    order += res(dec.mid.block_2) + attn(dec.mid.attn_1) + res(dec.mid.block_1) + [dec.conv_in]
-    q = model.quantize
-    books = list(q.embedding_list) if hasattr(q, "embedding_list") else [q.embedding]   # texture | plain quantizer
-    order += [model.post_quant_conv] + books + [model.quant_conv]
-    order += [enc.conv_out, enc.norm_out] + res(enc.mid.block_2) + attn(enc.mid.attn_1) + res(enc.mid.block_1)
+                order += _attn_order(lvl.attn[i_block])
+            order += _res_order(lvl.block[i_block])
+    return order
+
+
+def encoder_order(enc):
+    """leaf modules of an Encoder in backward-completion order"""
+    order = [enc.conv_out, enc.norm_out] + mid_order(enc.mid)
     for i_level in reversed(range(enc.num_resolutions)):
         lvl = enc.down[i_level]
         if i_level != enc.num_resolutions - 1:
             order.append(lvl.downsample.conv)
         for i_block in reversed(range(enc.num_res_blocks)):
             if len(lvl.attn) > 0:
-                order += attn(lvl.attn[i_block])
-            order += res(lvl.block[i_block])
+                order += _attn_order(lvl.attn[i_block])
+            order += _res_order(lvl.block[i_block])
     order.append(enc.conv_in)
     return order
+
+
+def backward_order(model, disc=None):
+    """leaf modules of the generator in the order the backward pass finishes their gradients"""
+    dec = model.decoder
+    order = [dec.conv_out, dec.norm_out] + decoder_up_order(dec, dec.num_resolutions - 1)
+    order += mid_order(dec.mid) + [dec.conv_in]
+    q = model.quantize
+    books = list(q.embedding_list) if hasattr(q, "embedding_list") else [q.embedding]   # texture | plain quantizer
+    order += [model.post_quant_conv] + books + [model.quant_conv]
+    return order + encoder_order(model.encoder)
 
 
 # ----------------------------------------------------------------------------
@@ -517,6 +549,7 @@ class DiscNet(Layer):
 class VQGANTrainer:
     """Owns a ``pipeline.VQImageSegmTextureModel`` (encoder, decoder, quantize, quant_conv, post_quant_conv) and a
     ``Discriminator``; ``optimize_parameters(data, step)`` is one reference training step."""
+    fixed = None
 
     def __init__(self, model, disc, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, disc_start_step=0, disc_weight_max=1.0,
                  perceptual_weight=1.0, diff_aug=True, beta=0.25, micro_batch=None, bucket_bytes=48 << 20):
@@ -527,21 +560,20 @@ class VQGANTrainer:
         self.micro_batch = micro_batch
         self.device = next(model.parameters()).device
         dev = self.device
-        self.enc_in, self.enc_body, self.enc_out = encoder_layers(self, model.encoder)
-        self.dec_in, self.dec_body, self.dec_out = decoder_layers(self, model.decoder)
-        self.qconv, self.pqconv = Lin1x1L(self, model.quant_conv), Lin1x1L(self, model.post_quant_conv)
+        order, self.quantizer = self._build(model, bucket_bytes)
         self.dnet = DiscNet(self, disc)
-        self.gen = ParamSpace(backward_order(model), dev, bucket_bytes)
+        self.gen = ParamSpace(order, dev, bucket_bytes)
         self.dsc = ParamSpace(self.dnet.order(), dev, bucket_bytes)
+        self.spaces = [sp for sp in (self.gen, self.dsc, self.fixed) if sp is not None]
         self._space = {}
-        for sp in (self.gen, self.dsc):
+        for sp in self.spaces:
             for mod, _, _ in sp.mod_span:
                 self._space[mod] = sp
         self._pspace = {}
-        for sp in (self.gen, self.dsc):
+        for sp in self.spaces:
             for p, _, _ in sp.slots:
                 self._pspace[id(p)] = sp
-        ws = [e.weight for e in model.quantize.embedding_list]
+        ws = [e.weight for e in self.quantizer.embedding_list]
         n_e, D = ws[0].shape
         cb, gcb = self.gen.joint(ws, D)
         self.codebook, self.g_codebook = cb.view(18, n_e, D), gcb.view(18, n_e, D)
@@ -549,6 +581,14 @@ class VQGANTrainer:
         self.aug_draw_fn = None     # tests inject the reference's recorded DiffAugment draws here
         self.log = {}
         self._sync_from_rank0()
+
+    def _build(self, model, bucket_bytes):
+        """the generator's layers -> (its stepped modules in backward-completion order, its texture quantizer); a
+        subclass may also set ``fixed``, a ParamSpace of modules whose gradients are computed but never stepped"""
+        self.enc_in, self.enc_body, self.enc_out = encoder_layers(self, model.encoder)
+        self.dec_in, self.dec_body, self.dec_out = decoder_layers(self, model.decoder)
+        self.qconv, self.pqconv = Lin1x1L(self, model.quant_conv), Lin1x1L(self, model.post_quant_conv)
+        return backward_order(model), model.quantize
 
     # ---- plumbing used by the layers
     def space_of(self, mod):
@@ -602,7 +642,7 @@ class VQGANTrainer:
         nel = z.numel()
         dz = ops.vq_bwd(z, self.codebook, idx, ids, g.g, self.g_codebook, 2.0 * cb_scale / nel,
                         2.0 * self.beta * cb_scale / nel)
-        for e in self.model.quantize.embedding_list:
+        for e in self.quantizer.embedding_list:
             self.gen.done(e)
         g = self.qconv.bwd(Grad(dz))
         self.enc_in.bwd(self.enc_body.bwd(self.enc_out.bwd(g.g)))
@@ -671,16 +711,15 @@ class VQGANTrainer:
         self.loss_scale = 2.0 ** math.floor(math.log2(nel))
         self.disc_scale = 2.0 ** 14
         self.n_micro = n_micro
-        self.gen.flat_g.zero_()
-        self.dsc.flat_g.zero_()
-        self.gen.prepare(terms)
-        self.dsc.prepare(terms)
+        for sp in self.spaces:
+            sp.flat_g.zero_()
+            sp.prepare(terms)
         outs = []
         for i in range(n_micro):
             outs.append(self._micro_step(x[i * mb:(i + 1) * mb], mask[i * mb:(i + 1) * mb], step, n_micro,
                                          i == n_micro - 1, generator))
-        self.gen.release()
-        self.dsc.release()
+        for sp in self.spaces:
+            sp.release()
         self._outs = outs
         self._did_disc = step > self.disc_start_step
         return outs
