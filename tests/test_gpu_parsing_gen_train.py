@@ -294,6 +294,9 @@ def test_native_step_full_gradients_second_shape(cuda):
 
 
 def test_native_step_real_widths(cuda):
+    """The whole step at the real widths keeps the spread-based bar of _compare_full: the ShapeUNet's arithmetic at
+    these widths, with kink flips ruled out, is held to 5e-4 against conditioned fp64 by
+    tests/test_gpu_train_layers.py."""
     _ops()
     tr, sds = build(cuda, cfgs=REAL)
     data = PT.batch(PT.TRAIN_SEEDS, (2, 128, 64))
