@@ -565,6 +565,32 @@ int t2h_routed_head_ce(const float* y, const int64_t* tex, const int64_t* own, c
                        int64_t m, int g, int c, int ncls, float gscale, double* loss_sum, float* dy, float* dw,
                        float* db, int32_t* order, int32_t* off, float* dl, t2h_stream_t stream);
 
+/* ------------------------------------------------------------------------
+ * LPIPS perceptual loss (lpips==0.1.4, net='vgg', version='0.1'; models/vqgan_model.py:427,450,
+ * models/hierarchy_vqgan_model.py:90,253).  The VGG16 convolutions and their data gradients run on t2h_tapgemm.
+ * ---------------------------------------------------------------------- */
+/* ScalingLayer of two fp32 NCHW image batches x0, x1 [b][3][h][w]: out = fp16 planes [terms][2b][h][w][8] of
+ * (x - shift[c]) / scale[c] (images [0,b) from x0, [b,2b) from x1; channels 3..7 zero).  shift, scale: 3 floats */
+int t2h_lpips_scale_fwd(const float* x0, const float* x1, const float* shift, const float* scale, void* out, int b,
+                        int h, int w, int terms, t2h_stream_t stream);
+/* adjoint of the ScalingLayer: g[n][c][h][w] += alpha * d[n][h][w][c] / scale[c] for c < 3; d fp32 NHWC with row
+ * stride ld (conv1_1's data gradient), g fp32 NCHW [b][3][h][w] */
+int t2h_lpips_scale_bwd(const float* d, int ld, const float* scale, float alpha, float* g, int b, int h, int w,
+                        t2h_stream_t stream);
+/* One fused LPIPS head over a slice's features f0 (from in0) and f1 (from in1), fp32 NHWC [b][h][w][c]:
+ * d = sum_c w_c (f0_c/(|f0|+1e-10) - f1_c/(|f1|+1e-10))^2 per pixel; sum[n] += inv_hw * sum over the image's pixels
+ * of d, summed in a fixed order.  With planes (fp16 [terms][b][h][w][c]): planes = (f1 > 0) * (gin + gscale *
+ * dd/df1), the gradient at the pre-activation of the slice's last conv (gin fp32 NHWC like f1, or NULL: 0).
+ * ws: t2h_lpips_head_chunks(h, w) * b doubles of scratch.  c % 4 == 0, c <= 512. */
+int t2h_lpips_head(const float* f0, const float* f1, const float* w, const float* gin, int b, int h, int w_, int c,
+                   float inv_hw, float gscale, double* sum, double* ws, void* planes, int terms, t2h_stream_t stream);
+/* number of per-image partial sums t2h_lpips_head writes to its ws */
+int t2h_lpips_head_chunks(int h, int w);
+/* dpre planes [terms][n] = dy * (y > 0), y = ReLU(pre) given by the hi plane of its fp16 planes (as t2h_lrelu_bwd:
+ * 0 < y <= 2^-25 rounds to an fp16 0 and passes no gradient); n % 8 == 0 */
+int t2h_relu_bwd(const void* y_planes, const float* dy, void* dpre_planes, int terms, int64_t n,
+                 t2h_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

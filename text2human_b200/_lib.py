@@ -131,6 +131,11 @@ SIGNATURES = {
     "t2h_ce_logits": (_I, [_P, _P, _I, _I, _I, _I, _I, _F, _P, _P, _I, _P, _P]),
     "t2h_shape_attr_embed_bwd": (_I, [_P] * 13 + [_I, _I, _I, _I, _P]),
     "t2h_routed_head_ce": (_I, [_P, _P, _P, _P, _P, _L, _I, _I, _I, _F, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "t2h_lpips_scale_fwd": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "t2h_lpips_scale_bwd": (_I, [_P, _I, _P, _F, _P, _I, _I, _I, _P]),
+    "t2h_lpips_head": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _P, _P, _P, _I, _P]),
+    "t2h_lpips_head_chunks": (_I, [_I, _I]),
+    "t2h_relu_bwd": (_I, [_P, _P, _P, _I, _L, _P]),
     "t2h_sample_step": (_I, [_P, _P, _P, _P, _P, _L, _I, _I, _F, _F, C.c_uint64, C.c_uint32, _L, _P]),
 }
 

@@ -1481,3 +1481,60 @@ def routed_head_ce(y, tex, own, w, b, loss_sum, dw, db, gscale=1.0):
                                               gscale, _ptr(loss_sum), _ptr(dy), _ptr(dw), _ptr(db), _ptr(order),
                                               _ptr(off), _ptr(dl), _stream()))
     return dy
+
+
+# ----------------------------------------------------------------------------
+# LPIPS (lpips==0.1.4, net='vgg'): input scaling, fused per-slice head, ReLU backward (csrc/lpips.cu)
+# ----------------------------------------------------------------------------
+def lpips_scale_fwd(x0, x1, shift, scale, terms=None):
+    """ScalingLayer of two fp32 NCHW batches [B,3,H,W] -> planes [T,2B,H,W,8]: in0's images first, then in1's"""
+    _need_cuda(x0, x1, shift, scale)
+    x0, x1 = _f32c(x0), _f32c(x1)
+    B, Cc, H, W = x1.shape
+    assert x0.shape == x1.shape and Cc == 3 and shift.numel() == 3 and scale.numel() == 3
+    terms = terms or get_terms()
+    out = torch.empty((terms, 2 * B, H, W, 8), dtype=torch.float16, device=x1.device)
+    _count(1)
+    _lib.check(_lib.load().t2h_lpips_scale_fwd(_ptr(x0), _ptr(x1), _ptr(_f32c(shift)), _ptr(_f32c(scale)), _ptr(out),
+                                               B, H, W, terms, _stream()))
+    return out
+
+
+def lpips_scale_bwd(d, scale, alpha, g):
+    """g fp32 NCHW [B,3,H,W] += alpha * d[..., :3] / scale (d: conv1_1's data gradient, fp32 NHWC [B,H,W,ld])"""
+    _need_cuda(d, scale, g)
+    B, H, W, ld = d.shape
+    assert d.is_contiguous() and g.is_contiguous() and g.dtype == torch.float32 and g.shape == (B, 3, H, W)
+    _count(1)
+    _lib.check(_lib.load().t2h_lpips_scale_bwd(_ptr(d), ld, _ptr(_f32c(scale)), alpha, _ptr(g), B, H, W, _stream()))
+    return g
+
+
+def lpips_head(f0, f1, w, sum_out, *, gscale=0.0, gin=None, want_grad=True, terms=None):
+    """One LPIPS head over the slice features f0 (in0) / f1 (in1), fp32 NHWC [B,h,w,C]: sum_out fp64 [B] += the
+    spatial mean of sum_c w_c (unit(f0)_c - unit(f1)_c)^2; -> planes [T,B,h,w,C] of (f1 > 0) * (gin + gscale *
+    d(per-pixel d)/df1) (or None without ``want_grad``)"""
+    _need_cuda(f0, f1, w, sum_out)
+    B, H, W, Cc = f1.shape
+    assert f0.shape == f1.shape and f0.is_contiguous() and f1.is_contiguous() and w.numel() == Cc
+    assert sum_out.dtype == torch.float64 and sum_out.numel() == B
+    assert gin is None or (want_grad and gin.shape == f1.shape and gin.is_contiguous())
+    lib = _lib.load()
+    terms = terms or get_terms()
+    planes = torch.empty((terms, B, H, W, Cc), dtype=torch.float16, device=f1.device) if want_grad else None
+    ws = torch.empty((B * lib.t2h_lpips_head_chunks(H, W),), dtype=torch.float64, device=f1.device)
+    _count(2)
+    _lib.check(lib.t2h_lpips_head(_ptr(f0), _ptr(f1), _ptr(_f32c(w)), _ptr(gin), B, H, W, Cc, 1.0 / (H * W), gscale,
+                                  _ptr(sum_out), _ptr(ws), _ptr(planes), terms, _stream()))
+    return planes
+
+
+def relu_bwd(y_hi, dy, terms=None):
+    """dpre = dy * (y > 0) -> planes [T, *dy.shape]; y_hi: the hi plane of y = ReLU(pre), shaped like dy"""
+    _need_cuda(y_hi, dy)
+    assert y_hi.shape == dy.shape and y_hi.is_contiguous() and dy.is_contiguous() and dy.dtype == torch.float32
+    terms = terms or get_terms()
+    out = torch.empty((terms,) + tuple(dy.shape), dtype=torch.float16, device=dy.device)
+    _count(1)
+    _lib.check(_lib.load().t2h_relu_bwd(_ptr(y_hi), _ptr(dy), _ptr(out), terms, dy.numel(), _stream()))
+    return out

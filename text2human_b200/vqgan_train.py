@@ -5,8 +5,9 @@ Mirrors ``VQImageSegmTextureModel.training_step`` / ``optimize_parameters`` (mod
 with ``models/losses/vqgan_loss.py`` (adaptive weight :5-12, hinge :21-26, DiffAugment 'color,translation' :29-80),
 ``Discriminator`` (models/archs/vqgan_arch.py:1155-1203, BatchNorm in training mode) and the straight-through /
 legacy-beta codebook loss of ``VectorQuantizerTexture.forward`` (:270-281); ``loss.backward()`` is replaced by the
-explicit backward below.  LPIPS (lpips==0.1.4, VGG weights: unavailable offline) is stubbed to zero, as BASELINE
-config 5 prescribes.
+explicit backward below.  The perceptual term ``perceptual_weight * LPIPS(x, xrec)`` (vqgan_model.py:450-451) runs when
+an ``lpips.LPIPS`` module is passed as ``perceptual=``; without one it is zero (BASELINE config 5, where the lpips
+package and its VGG weights are not available).
 
 Every dense contraction runs on the wgmma tap-GEMM: forward convs, data gradients (the forward kernel on transposed
 weight planes with negated taps; four parity launches for the strided convs), weight gradients (``t2h_conv_wgrad``:
@@ -552,8 +553,12 @@ class VQGANTrainer:
     fixed = None
 
     def __init__(self, model, disc, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, disc_start_step=0, disc_weight_max=1.0,
-                 perceptual_weight=1.0, diff_aug=True, beta=0.25, micro_batch=None, bucket_bytes=48 << 20):
+                 perceptual_weight=1.0, diff_aug=True, beta=0.25, micro_batch=None, bucket_bytes=48 << 20,
+                 perceptual=None):
+        """``perceptual``: a ``text2human_b200.lpips.LPIPS`` (frozen) adding ``perceptual_weight`` x LPIPS(x, xrec) to
+        nll_loss, as the reference does; None: the perceptual term is zero"""
         self.model, self.disc = model, disc
+        self.perceptual, self.perceptual_weight = perceptual, perceptual_weight
         self.lr, self.betas, self.eps = lr, betas, eps
         self.disc_start_step, self.disc_weight_max = disc_start_step, disc_weight_max
         self.diff_aug, self.beta = diff_aug, beta
@@ -654,11 +659,16 @@ class VQGANTrainer:
         dev = x.device
         S = self.loss_scale
         reduce = last and not self.force_no_reduce      # buckets fire during the LAST micro-batch's backward only
-        acc = torch.zeros(8, dtype=torch.float64, device=dev)   # l1 sum, fake-logit sum, sqerr, hinge real, hinge fake
+        # l1 sum, fake-logit sum, -, hinge real, hinge fake, -, -, -, then B perceptual values
+        acc = torch.zeros(8 + B, dtype=torch.float64, device=dev)
         dw = torch.zeros(1, dtype=torch.float32, device=dev)
         xrec, sqerr, z_numel = self.gen_forward(x, mask)
         nel = xrec.numel()
         g_nll = ops.l1_loss(x, xrec, acc[0:1], gscale=S / nel)
+        if self.perceptual is not None:
+            # nll = mean(|x - xrec| + w * p_loss[b]) over [B,3,H,W]: d nll / d p_loss[b] = w / B; the trunk's
+            # activations are freed here, before the discriminator's exist
+            acc[8:] = self.perceptual.run(x, xrec, g=g_nll, alpha=self.perceptual_weight * S / B)
         if self.diff_aug:
             r, t = self._aug_draws(B, H, W, dev, generator)
             xr = ops.diffaug_fwd(xrec, r, t)
@@ -728,11 +738,14 @@ class VQGANTrainer:
         """the reference's logged scalars (one device->host read; means over the micro-batches)"""
         o = self._outs
         n = len(o)
-        nll = sum(float(r["acc"][0]) / r["nel"] for r in o) / n
+        l1 = sum(float(r["acc"][0]) / r["nel"] for r in o) / n
+        p = sum(float(r["acc"][8:].mean()) for r in o) / n
+        nll = l1 + self.perceptual_weight * p
         g_loss = -sum(float(r["acc"][1]) / r["n_logit"] for r in o) / n
         cb = sum((1.0 + self.beta) * float(r["sqerr"][0]) / r["z_numel"] for r in o) / n
         dw = sum(float(r["dw"][0]) for r in o) / n
-        out = dict(nll_loss=nll, g_loss=g_loss, codebook_loss=cb, d_weight=dw, loss=nll + dw * g_loss + cb)
+        out = dict(nll_loss=nll, g_loss=g_loss, codebook_loss=cb, d_weight=dw, loss=nll + dw * g_loss + cb, l1=l1,
+                   perceptual=p)
         if self._did_disc:
             out["d_loss"] = sum(0.5 * (float(r["acc"][3]) + float(r["acc"][4])) / r["n_dlogit"] for r in o) / n
         return out
