@@ -55,6 +55,59 @@ def lpips(sd, in0, in1):
     return val
 
 
+def pool_windows(x):
+    """[N,C,H,W] -> [N,C,H/2,W/2,4]: each 2x2 window of MaxPool2d(2) row-major (torch's order of first maxima)"""
+    N, C, H, W = x.shape
+    return x.reshape(N, C, H // 2, 2, W // 2, 2).permute(0, 1, 2, 4, 3, 5).reshape(N, C, H // 2, W // 2, 4)
+
+
+def choices(sd, in0, in1):
+    """the discrete choices of an fp64 forward of the 2B images (in0's first): (masks, picks) as
+    ``lpips_conditioned`` takes them -- pre-activation > 0 per conv, first maximum per max-pool window"""
+    shift, scale = sd["scaling_layer.shift"], sd["scaling_layer.scale"]
+    h = torch.cat([(in0 - shift) / scale, (in1 - shift) / scale])
+    masks, picks = [], []
+    for k, idxs in enumerate(CONV_IDX):
+        if k > 0:
+            picks.append(pool_windows(h).argmax(-1))
+            h = F.max_pool2d(h, kernel_size=2, stride=2)
+        for i in idxs:
+            p = _slice_key(i)
+            u = F.conv2d(h, sd[p + ".weight"], sd[p + ".bias"], padding=1)
+            masks.append(u > 0)
+            h = F.relu(u)
+    return masks, picks
+
+
+def lpips_conditioned(sd, in0, in1, masks, picks, trace=None):
+    """``lpips`` with every discrete choice imposed: conv i's ReLU multiplies by ``masks[i]`` (bool [2B,C,h,w], the 13
+    convs in CONV_IDX order, in0's images first) and the max-pool before slice k+2 takes the window element at
+    ``picks[k]`` (int [2B,C,h/2,w/2] in 0..3, row-major).  Away from every kink and tie, with fp64's own choices
+    (``choices``), this is ``lpips``.  -> [B,1,1,1], autograd-capable; ``trace`` (a list) receives, in order, each
+    max-pool's input and each conv's (input, pre-activation)."""
+    shift, scale = sd["scaling_layer.shift"], sd["scaling_layer.scale"]
+    B = in1.shape[0]
+    h = torch.cat([(in0 - shift) / scale, (in1 - shift) / scale])
+    outs, m = [], iter(masks)
+    for k, idxs in enumerate(CONV_IDX):
+        if k > 0:
+            if trace is not None:
+                trace.append(h.detach())
+            h = pool_windows(h).gather(-1, picks[k - 1].unsqueeze(-1)).squeeze(-1)
+        for i in idxs:
+            p = _slice_key(i)
+            u = F.conv2d(h, sd[p + ".weight"], sd[p + ".bias"], padding=1)
+            if trace is not None:
+                trace.append((h.detach(), u.detach()))
+            h = u * next(m).to(u.dtype)
+        outs.append(h)
+    val = 0
+    for k in range(5):
+        d = (normalize_tensor(outs[k][:B]) - normalize_tensor(outs[k][B:])) ** 2
+        val = val + F.conv2d(d, sd[f"lin{k}.model.1.weight"]).mean([2, 3], keepdim=True)
+    return val
+
+
 class LPIPSRef(torch.nn.Module):
     """nn.Module wrapper of ``lpips`` on a fixed state dict (the reference step calls ``self.perceptual(x, xrec)``)"""
 

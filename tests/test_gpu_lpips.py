@@ -39,9 +39,12 @@ def _inputs(cuda, B, H, W, seed):
 
 # The gradient is discontinuous at every ReLU kink and max-pool tie of the trunk: an element whose pre-activation (or
 # window runner-up) lies within rounding of the kink lands on either side in any fp32 computation, and moves a whole
-# gradient element.  Plain torch fp32 on the CPU already differs from fp64 by 1.8e-4 (norm) / 7.8e-3 (worst element)
-# at 3 x 256 x 128 on this recipe; the native fp32 mode was measured at 3.1e-4 / 1.3e-3 (2 x 64 x 32) and
-# 1.2e-3 / 3.4e-2 (3 x 256 x 128) on an H100 80GB HBM3 (700 W), independent of the gradient planes' scale.
+# gradient element.  That is the whole gap measured here on an H100 80GB HBM3 (700 W): 3.1e-4 (norm) / 1.3e-3 (worst
+# element) at 2 x 64 x 32 and 1.2e-3 / 3.4e-2 at 3 x 256 x 128.  test_gpu_lpips_kernels.py::
+# test_lpips_stages_and_conditioned runs the same inputs against the fp64 restatement conditioned on the native ReLU
+# masks and max-pool picks: the gradient then agrees to 5e-6, and the elements whose mask differs from fp64's sign
+# (5 at 2 x 64 x 32, within 1.4 fp32 rounding units of their kink; 74 masks and 16 picks at 3 x 256 x 128, within 30)
+# are rounding-level kink flips.  The value is a fixed-order fp64 sum of fp32 per-pixel terms: within 3.1e-7.
 @pytest.mark.parametrize("B,H,W,gtol,wtol", [(2, 64, 32, 1e-3, 3e-3), (3, 256, 128, 3e-3, 6e-2)])
 def test_value_and_gradient_match_fp64(cuda, B, H, W, gtol, wtol):
     from text2human_b200 import ops
@@ -55,7 +58,7 @@ def test_value_and_gradient_match_fp64(cuda, B, H, W, gtol, wtol):
     gnorm = float((g - wg).norm() / wg.norm())
     gmax = float((g - wg).abs().max() / wg.abs().max())
     print(f"[lpips {B}x{H}x{W}] value rel {verr:.2e}, grad norm rel {gnorm:.2e}, worst element / largest {gmax:.2e}")
-    assert verr <= 1e-4 and gnorm <= gtol and gmax <= wtol, (verr, gnorm, gmax)
+    assert verr <= 1e-6 and gnorm <= gtol and gmax <= wtol, (verr, gnorm, gmax)
     # the no_grad path (forward only) gives the same values
     with torch.no_grad():
         v2 = m(in0, in1).double().cpu()

@@ -101,6 +101,37 @@ def test_rejected_inputs_before_any_launch():
         m(x, x)
 
 
+def test_conditioned_restatement_with_fp64_choices_is_lpips():
+    """lpips_conditioned fed fp64's own ReLU signs and first-maximum positions reproduces lpips, value and in1
+    gradient, to 1e-12: the oracle the GPU tests condition on the native masks is LPIPS away from the kinks"""
+    sd = {k: v.double() for k, v in LR.state_dict().items()}
+    g = torch.Generator().manual_seed(5)
+    x0 = torch.rand((2, 3, 32, 48), generator=g, dtype=torch.float64) * 2 - 1
+    x1 = torch.rand((2, 3, 32, 48), generator=g, dtype=torch.float64) * 2 - 1
+    res = []
+    for cond in (False, True):
+        x = x1.clone().requires_grad_(True)
+        if cond:
+            masks, picks = lpips_ref.choices(sd, x0, x1)
+            assert len(masks) == 13 and len(picks) == 4 and masks[0].shape == (4, 64, 32, 48)
+            trace = []
+            v = lpips_ref.lpips_conditioned(sd, x0, x, masks, picks, trace)
+            assert len(trace) == 17
+        else:
+            v = lpips_ref.lpips(sd, x0, x)
+        v.sum().backward()
+        res.append((v.detach(), x.grad))
+    (v, gr), (vc, gc) = res
+    assert v.shape == vc.shape == (2, 1, 1, 1)
+    assert float(((vc - v).abs() / v.abs()).max()) <= 1e-12
+    assert float((gc - gr).abs().max() / gr.abs().max()) <= 1e-12
+    # a flipped mask element changes the result: the masks are used, not recomputed
+    masks[1] = masks[1].clone()
+    masks[1][3, :, 10:14, 20:30] = ~masks[1][3, :, 10:14, 20:30]
+    vf = lpips_ref.lpips_conditioned(sd, x0, x1, masks, picks)
+    assert float(((vf - v).abs() / v.abs()).max()) > 1e-6
+
+
 def test_restatement_dead_pixels_give_finite_gradient():
     """relu5_3 zero everywhere: torch's threshold_backward masks the NaN of sqrt's backward at 0"""
     sd = {k: v.double() for k, v in LR.state_dict(dead_slice5=True).items()}

@@ -23,6 +23,15 @@ constexpr int kHeadWarps = 8;
 constexpr int kHeadMaxC = 512;
 constexpr int kHeadQ = kHeadMaxC / 128;  // float4 slots per lane
 
+// The largest fp32 whose hi/lo split is finite (65520 rounds to an fp16 inf).  A gradient beyond it would split into
+// hi = +inf, lo = -inf, whose sum in the next contraction is NaN; it is saturated here instead (NaN stays NaN).
+// Every value whose split was finite is split exactly as before.
+constexpr float kSplitMax = 65519.99609375f;
+
+__device__ __forceinline__ void split_f16_sat(float v, __half& hi, __half& lo) {
+  split_f16(fabsf(v) > kSplitMax ? copysignf(kSplitMax, v) : v, hi, lo);
+}
+
 }  // namespace
 
 // (x - shift[c]) / scale[c] of two fp32 NCHW images [b][3][hw] -> planes [terms][2b][hw][8]: images [0,b) from x0,
@@ -72,6 +81,9 @@ __global__ void lpips_scale_bwd_kernel(const float* __restrict__ d, int ld, cons
 // and the planes [terms][b][hw][c] get (f1_j > 0) * (gin_j + gscale * dd/df1_j): the gradient at the
 // pre-activation of the slice's last conv.  Where f1_j > 0, |f1| > 0, so the masked expression is finite; every
 // other element is written 0 (torch's threshold_backward masks the NaN of sqrt's backward at an all-zero pixel).
+// dd/df1 grows like 1/|f1|: at a pixel whose |f1| is tiny but not 0 (of order 1e-6 at slice 1) the scaled gradient
+// passes fp16's range, and it is saturated at kSplitMax (split_f16_sat) -- the one place where the planes deviate
+// from the exact gradient by more than rounding.
 __global__ void __launch_bounds__(kHeadWarps * 32)
 lpips_head_kernel(const float* __restrict__ f0, const float* __restrict__ f1, const float* __restrict__ w,
                   const float* __restrict__ gin, long long hw, int c, float gscale, double* __restrict__ ws,
@@ -140,7 +152,7 @@ lpips_head_kernel(const float* __restrict__ f0, const float* __restrict__ f1, co
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const float r = fv[e] > 0.f ? gx[e] + gscale * (gg[e] * i1 - fv[e] * k2) : 0.f;
-          split_f16(r, hi[e], lo[e]);
+          split_f16_sat(r, hi[e], lo[e]);
         }
         const long long off = base + 4LL * q;
         *reinterpret_cast<uint2*>(planes + off) = *reinterpret_cast<const uint2*>(hi);
@@ -168,7 +180,8 @@ __global__ void lpips_head_sum_kernel(const double* __restrict__ ws, int chunks,
 }
 
 // planes[t][i] = split(dy[i] * (y[i] > 0)), y = ReLU(pre) given by the hi plane of its fp16 planes (the rule of
-// lrelu_bwd_kernel: 0 < y <= 2^-25 rounds to an fp16 0 and passes no gradient).  8 elements per thread.
+// lrelu_bwd_kernel: 0 < y <= 2^-25 rounds to an fp16 0 and passes no gradient), saturated as the head's planes are
+// (a saturated head gradient can carry a data gradient past fp16's range).  8 elements per thread.
 __global__ void relu_bwd_kernel(const __half* __restrict__ y, const float* __restrict__ dy, __half* __restrict__ out,
                                 int terms, long long n8) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8;
@@ -180,7 +193,7 @@ __global__ void relu_bwd_kernel(const __half* __restrict__ y, const float* __res
     const float dv[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
     __align__(16) __half hi[8], lo[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) split_f16(__half2float(yh[e]) > 0.f ? dv[e] : 0.f, hi[e], lo[e]);
+    for (int e = 0; e < 8; ++e) split_f16_sat(__half2float(yh[e]) > 0.f ? dv[e] : 0.f, hi[e], lo[e]);
     reinterpret_cast<uint4*>(out)[i] = *reinterpret_cast<const uint4*>(hi);
     if (terms == 2) reinterpret_cast<uint4*>(out)[n8 + i] = *reinterpret_cast<const uint4*>(lo);
   }

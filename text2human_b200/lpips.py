@@ -17,6 +17,11 @@ Because the loss is a scalar per image and in0 is constant, the gradient with re
 call as the value ("gradient at forward"): every head folds its own backward and the mask of its slice's last ReLU
 into one pass, and the data gradients walk the trunk back to the image.  The autograd node only scales that map by
 ``grad_output[b]``, so it can run its backward any number of times (``retain_graph``).
+
+Deviation: a head's gradient grows like 1/|f1| at a pixel whose xrec features are tiny but not all zero (|f1| of
+order 1e-6 at slice 1).  Where the scaled gradient passes fp16's range (65520) the head and the ReLU backward saturate
+it instead of writing inf planes, whose hi + lo would be NaN in every gradient downstream; the image gradient stays
+finite but is no longer the exact one at such pixels.  Every value within range is unchanged.
 """
 import math
 
