@@ -62,12 +62,14 @@ def disc_kink_margin(sd, x, n_layers=3):
 
 
 def training_step(sd, top_books, bot_books, sd_disc, x, mask, step, *, disc_start_step=1, disc_weight_max=1.0,
-                  diff_aug=True, disc_layers=3, probe=None):
+                  diff_aug=True, disc_layers=3, probe=None, disc_masks=None):
     """-> dict(loss, d_loss or None, nll_loss, g_loss, d_weight, codebook_loss, bot_idx, xrec).  sd keys:
     top_encoder.*, top_quant_conv.*, top_post_quant_conv.*, decoder.*, bot_encoder.*, bot_quant_conv.*,
     bot_post_quant_conv.*, bot_decoder_res.*; top_books [18, 1024, D] (frozen), bot_books: 18 [n_e, 4 D] (requires
     grad for the codebook gradient).  ``probe`` (dict): 'argmin' (relative second-best gaps of both quantizers) and
-    'kink' (discriminator margins of the three passes) for the fixture's seed scan."""
+    'kink' (discriminator margins of the three passes) for the fixture's seed scan.  ``disc_masks``: per
+    discriminator pass the LeakyReLU masks TR.discriminator imposes (fake image, real image, detached fake image)."""
+    masks = list(disc_masks) if disc_masks is not None else [None] * 3
     with torch.no_grad():                                                   # forward_step :236-237
         ht = V.conv(sd, "top_quant_conv", V.encoder(sd, x, "top_encoder."), padding=0)
         quant_top, _, _, _ = V.quantize_texture(top_books, ht, mask)
@@ -84,7 +86,7 @@ def training_step(sd, top_books, bot_books, sd_disc, x, mask, step, *, disc_star
     # training_step :253-291, as the top step (oracle/vqgan_train_ref.training_step)
     nll_loss = torch.mean(torch.abs(x - xrec))
     xr = TR.diff_augment(xrec) if diff_aug else xrec
-    g_loss = -torch.mean(TR.discriminator(sd_disc, xr, n_layers=disc_layers))
+    g_loss = -torch.mean(TR.discriminator(sd_disc, xr, n_layers=disc_layers, masks=masks[0]))
     last = sd["decoder.conv_out.weight"]
     rg = torch.autograd.grad(nll_loss, last, retain_graph=True)[0]
     gg = torch.autograd.grad(g_loss, last, retain_graph=True)[0]
@@ -94,8 +96,8 @@ def training_step(sd, top_books, bot_books, sd_disc, x, mask, step, *, disc_star
     d_loss = None
     if step > disc_start_step:
         real_in = TR.diff_augment(x.detach()) if diff_aug else x.detach()
-        lr_ = TR.discriminator(sd_disc, real_in, n_layers=disc_layers)
-        lf_ = TR.discriminator(sd_disc, xr.detach(), n_layers=disc_layers)
+        lr_ = TR.discriminator(sd_disc, real_in, n_layers=disc_layers, masks=masks[1])
+        lf_ = TR.discriminator(sd_disc, xr.detach(), n_layers=disc_layers, masks=masks[2])
         d_loss = 0.5 * (torch.mean(F.relu(1.0 - lr_)) + torch.mean(F.relu(1.0 + lf_)))
         if probe is not None:
             probe["kink"] = [disc_kink_margin(sd_disc, t.detach(), disc_layers) for t in (xr, real_in)]

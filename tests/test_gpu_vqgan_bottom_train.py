@@ -304,9 +304,12 @@ def test_invalid_inputs_raise_before_any_launch(cuda):
 
 
 # ---------------------------------------------------------------- real widths
-def test_real_width_step_against_fp64_restatement(cuda):
+def test_real_width_step_against_fp64_restatement(cuda, monkeypatch):
     """configs/vqvae_bottom.yml widths, B = 1, 512 x 256: the native fp32 step and the fp32 restatement, each against
-    the fp64 restatement on the GPU"""
+    the fp64 restatement on the GPU.  The generator's gradient through the discriminator is discontinuous at its
+    LeakyReLU kinks, some of which lie within rounding of a pre-activation at this size: both restatements take the
+    native step's own masks (recorded first), as test_gpu_vqgan_train_widths does."""
+    from test_gpu_vqgan_train_widths import disc_masks, record_disc_passes
     from oracle import vqgan_bottom_train_ref as BT
     from text2human_b200 import ops
     from text2human_b200.pipeline import HierarchyVQSpatialTextureAwareModel
@@ -331,6 +334,13 @@ def test_real_width_step_against_fp64_restatement(cuda):
     disc = Discriminator(3, 64, n_layers=3)
     disc.load_state_dict(R.fill_state_dict(R.spec_of(disc), seeds["disc"]), strict=True)
     x, mask = R.image(11, 1, 3, 512, 256), R.blocky_mask(12, 1, 512, 256, 32)
+    passes = record_disc_passes(monkeypatch)
+    tr = HierarchyVQGANTrainer(m.to(cuda), disc.to(cuda), disc_start_step=1, diff_aug=False)
+    tr.training_step(dict(image=x, texture_mask=mask), BR.STEP)
+    torch.cuda.synchronize()
+    got = tr.losses()
+    masks = disc_masks(passes)
+    del passes
     ref = {}
     for dt in (torch.float64, torch.float32):
         sd = {f"{n}.{k}": v.detach().to(cuda, dt).clone() for n in
@@ -344,15 +354,11 @@ def test_real_width_step_against_fp64_restatement(cuda):
         sdd = {k: (v.detach().to(cuda, dt).clone().requires_grad_("running" not in k) if v.is_floating_point()
                    else v.detach().to(cuda).clone()) for k, v in disc.state_dict().items()}
         r_ = BT.training_step(sd, top, bot, sdd, x.to(cuda, dt), mask.to(cuda), BR.STEP, disc_start_step=1,
-                              diff_aug=False)
+                              diff_aug=False, disc_masks=masks)
         r_["loss"].backward()
         ref[dt] = ({k: float(r_[k]) for k in ("nll_loss", "g_loss", "codebook_loss", "d_weight")},
                    {k: g.detach().double() for k, g in BR.gen_grads(sd, bot).items()}, r_["bot_idx"])
         del sd, sdd, bot, r_
-    tr = HierarchyVQGANTrainer(m.to(cuda), disc.to(cuda), disc_start_step=1, diff_aug=False)
-    tr.training_step(dict(image=x, texture_mask=mask), BR.STEP)
-    torch.cuda.synchronize()
-    got = tr.losses()
     named = named_gen(m)
     l64, g64, i64 = ref[torch.float64]
 
