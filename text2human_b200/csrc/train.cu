@@ -375,6 +375,110 @@ __global__ void ce_heads_kernel(const float* __restrict__ logits, const long lon
   if (tid == 0) loss_rows[m] = lse - lr[tgt];  // unweighted; the caller forms loss and vb_loss from it
 }
 
+// The 18 per-head logit gradients that torch's autograd hands to the sampler node: head k is a strided fp32
+// tensor [B][T][ncls] described by heads[k] = {pointer, stride_b, stride_t, stride_c} (elements; pointer 0 = all
+// zeros).  F.cross_entropy(logits.permute(0, 2, 1), ...) delivers them class-major (strides T*ncls, 1, T).
+struct HeadGrad {
+  long long ptr, sb, st, sc;
+};
+
+// largest |g| over every head -> *amax (bit pattern of a non-negative float, ordered like an unsigned int; a NaN
+// wins over inf, so the host sees it).  Dense heads (either layout) are read flat with 16-byte loads.
+__global__ void head_grads_absmax_kernel(const HeadGrad* __restrict__ heads, int B, int T, int ncls,
+                                         unsigned int* __restrict__ amax) {
+  const HeadGrad h = heads[blockIdx.y];
+  const float* x = reinterpret_cast<const float*>(h.ptr);
+  float m = 0.f;
+  bool nan = false;  // fmaxf drops a NaN operand, so NaNs are tracked on the side
+  if (x) {
+    const long long n = (long long)B * T * ncls;
+    const bool dense = (B == 1 || h.sb == (long long)T * ncls) &&
+                       ((h.st == ncls && h.sc == 1) || (h.st == 1 && h.sc == T));
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (dense && n % 4 == 0 && (h.ptr & 15) == 0) {
+      const float4* x4 = reinterpret_cast<const float4*>(x);
+      for (long long i = i0; i < n / 4; i += stride) {
+        const float4 v = x4[i];
+        m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+        nan |= v.x != v.x || v.y != v.y || v.z != v.z || v.w != v.w;
+      }
+    } else {
+      for (long long i = i0; i < n; i += stride) {
+        long long o = i;
+        if (!dense) {
+          const long long c = i % ncls, t = (i / ncls) % T, b = i / ((long long)ncls * T);
+          o = b * h.sb + t * h.st + c * h.sc;
+        }
+        const float v = x[o];
+        m = fmaxf(m, fabsf(v));
+        nan |= v != v;
+      }
+    }
+  }
+  unsigned int u = nan ? 0x7fc00000u : __float_as_uint(m);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) u = max(u, __shfl_xor_sync(0xffffffffu, u, o));
+  if ((threadIdx.x & 31) == 0 && u) atomicMax(amax, u);
+}
+
+// fp16 planes out[terms][B*T][nh*ncls] of scale*g, head k in columns [k*ncls, (k+1)*ncls): the operand of the heads'
+// weight- and data-gradient GEMMs.  One 64 (tokens) x 64 (classes) tile of one head of one image per block.  When the
+// token dimension is the contiguous one (the class-major layout the loss produces) the tile is read along tokens and
+// transposed through shared memory; otherwise it is read along classes.  The output is written along classes.
+__global__ void head_grads_to_planes_kernel(const HeadGrad* __restrict__ heads, int nh, int B, int T, int ncls,
+                                            float scale, int terms, __half* __restrict__ out) {
+  __shared__ float tile[64][65];  // [token][class]
+  const int k = blockIdx.z % nh, b = blockIdx.z / nh;
+  const int t0 = blockIdx.x * 64, c0 = blockIdx.y * 64;
+  const int tx = threadIdx.x, ty = threadIdx.y;  // 32 x 8
+  const HeadGrad h = heads[k];
+  const float* x = reinterpret_cast<const float*>(h.ptr);
+  if (x) x += (long long)b * h.sb;
+  if (x && h.st == 1 && h.sc != 1) {
+    for (int i = ty; i < 64; i += 8) {
+      const int c = c0 + i;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int t = t0 + tx + 32 * j;
+        tile[tx + 32 * j][i] = (c < ncls && t < T) ? x[(long long)c * h.sc + t] * scale : 0.f;
+      }
+    }
+  } else {
+    for (int i = ty; i < 64; i += 8) {
+      const int t = t0 + i;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int c = c0 + tx + 32 * j;
+        tile[i][tx + 32 * j] = (x && c < ncls && t < T) ? x[(long long)t * h.st + (long long)c * h.sc] * scale : 0.f;
+      }
+    }
+  }
+  __syncthreads();
+  const long long NK = (long long)nh * ncls;
+  const long long plane = (long long)B * T * NK;
+  const bool vec = (ncls & 1) == 0;  // every column pair then starts at an even offset
+  for (int i = ty; i < 64; i += 8) {
+    const int t = t0 + i, c = c0 + 2 * tx;
+    if (t >= T || c >= ncls) continue;
+    __half h0, l0, h1, l1;
+    split_f16(tile[i][2 * tx], h0, l0);
+    split_f16(tile[i][2 * tx + 1], h1, l1);
+    const long long o = ((long long)b * T + t) * NK + (long long)k * ncls + c;
+    if (vec) {
+      *reinterpret_cast<__half2*>(out + o) = __halves2half2(h0, h1);
+      if (terms == 2) *reinterpret_cast<__half2*>(out + plane + o) = __halves2half2(l0, l1);
+    } else {
+      out[o] = h0;
+      if (terms == 2) out[plane + o] = l0;
+      if (c + 1 < ncls) {
+        out[o + 1] = h1;
+        if (terms == 2) out[plane + o + 1] = l1;
+      }
+    }
+  }
+}
+
 // dE[idx[m]] += dx[m]  (embedding backward; also the positional table with idx = m % T)
 __global__ void embed_bwd_kernel(const float* __restrict__ dx, const long long* __restrict__ idx,
                                  float* __restrict__ dE, long long rows, int C, int T_mod) {
@@ -550,6 +654,31 @@ int t2h_ce_heads(const float* logits, const int64_t* target, const int64_t* head
   ce_heads_kernel<<<(unsigned)rows, 256, 0, as_stream(stream)>>>(
       logits, reinterpret_cast<const long long*>(target), reinterpret_cast<const long long*>(head), w, loss_rows,
       dlogits, nh, ncls);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_head_grads_absmax(const int64_t* heads, int nh, int b, int t, int ncls, float* amax, t2h_stream_t stream) {
+  T2H_CHECK_ARG(heads && amax && nh > 0 && nh <= 65535 && b > 0 && t > 0 && ncls > 0, "head_grads_absmax: bad args");
+  cudaStream_t st = as_stream(stream);
+  T2H_CUDA(cudaMemsetAsync(amax, 0, sizeof(float), st));
+  const long long n = (long long)b * t * ncls;
+  const int per_head = (int)std::max(1LL, std::min((long long)ceil_div64(n, 256 * 8), (long long)num_sms() * 4 / nh + 1));
+  head_grads_absmax_kernel<<<dim3(per_head, nh), 256, 0, st>>>(reinterpret_cast<const HeadGrad*>(heads), b, t, ncls,
+                                                               reinterpret_cast<unsigned int*>(amax));
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_head_grads_to_planes(const int64_t* heads, int nh, int b, int t, int ncls, float scale, int terms, void* out,
+                             t2h_stream_t stream) {
+  T2H_CHECK_ARG(heads && out && nh > 0 && b > 0 && t > 0 && ncls > 0, "head_grads_to_planes: bad args");
+  T2H_CHECK_ARG(terms == 1 || terms == 2, "head_grads_to_planes: terms=%d", terms);
+  T2H_CHECK_ARG((long long)nh * b <= 65535, "head_grads_to_planes: too many heads x images");
+  dim3 grid(ceil_div(t, 64), ceil_div(ncls, 64), nh * b), block(32, 8);
+  head_grads_to_planes_kernel<<<grid, block, 0, as_stream(stream)>>>(reinterpret_cast<const HeadGrad*>(heads), nh, b,
+                                                                     t, ncls, scale, terms,
+                                                                     reinterpret_cast<__half*>(out));
   T2H_LAUNCH_OK();
   return T2H_OK;
 }

@@ -956,6 +956,44 @@ def ce_heads(logits, target, head, w):
     return loss_rows, dlogits
 
 
+def head_grads_table(heads):
+    """the per-head gradients autograd hands over (fp32 [B, T, ncls] of any strides, or None for zeros) -> (device
+    int64 table [nh, 4] of (pointer, stride_b, stride_t, stride_c), (B, T, ncls)).  The tensors themselves are not
+    copied; the caller keeps them alive while the table is in use."""
+    ref = next(h for h in heads if h is not None)
+    _need_cuda(ref)
+    shape = tuple(ref.shape)
+    rows = []
+    for h in heads:
+        if h is None:
+            rows.append((0, 0, 0, 0))
+            continue
+        assert h.dtype == torch.float32 and tuple(h.shape) == shape and h.device == ref.device
+        rows.append((h.data_ptr(),) + tuple(h.stride()))
+    return torch.tensor(rows, dtype=torch.int64).to(ref.device), shape
+
+
+def head_grads_absmax(table, shape):
+    """-> fp32 [1] on the device: max |g| over every head of ``head_grads_table`` (NaN if any is NaN)"""
+    B, T, ncls = shape
+    amax = torch.empty((1,), dtype=torch.float32, device=table.device)
+    _count(1)
+    _lib.check(_lib.load().t2h_head_grads_absmax(_ptr(table), table.shape[0], B, T, ncls, _ptr(amax), _stream()))
+    return amax
+
+
+def head_grads_to_planes(table, shape, scale=1.0, terms=None):
+    """-> fp16 planes [T, B*T, nh*ncls] of scale*g, head k in columns [k*ncls, (k+1)*ncls): the same planes as
+    ``f32_to_planes_rows(scale * torch.cat(heads, -1).view(B*T, -1))``, read from the heads where they lie"""
+    B, T, ncls = shape
+    nh = table.shape[0]
+    terms = terms or get_terms()
+    out = torch.empty((terms, B * T, nh * ncls), dtype=torch.float16, device=table.device)
+    _count(1)
+    _lib.check(_lib.load().t2h_head_grads_to_planes(_ptr(table), nh, B, T, ncls, scale, terms, _ptr(out), _stream()))
+    return out
+
+
 def embed_bwd_(dE, dx, idx=None, t_mod=0):
     _need_cuda(dE, dx)
     rows, Cc = dx.shape

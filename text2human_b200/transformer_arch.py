@@ -5,7 +5,9 @@ reference (SURVEY.md §8b).  torch ``nn.Linear`` / ``nn.LayerNorm`` /
 ``nn.Embedding`` objects are parameter containers only; the arithmetic runs in
 libt2h: embedding-sum, LayerNorm, wgmma GEMMs (fused q|k|v projection, per-head
 q k^T and att v without head or v transposes, MLP with fused
-GELU, one N=18*1024 GEMM for the 18 heads), row softmax.
+GELU, one N=18*1024 GEMM for the 18 heads), row softmax.  While training (the
+reference's ``TransformerTextureAwareModel.optimize_parameters``) ``TransformerMultiHead.forward`` is one
+autograd node whose backward is ``transformer_train``'s hand-written one.
 
 The sampler is always non-causal on the Text2Human path (sampler='absorbing',
 transformer_arch.py:200,30), so no mask and no KV cache exist.
@@ -273,8 +275,14 @@ class TransformerMultiHead(nn.Module):
         out = ops.bmm_nt(hf_grouped.view(Tt, self.num_head, rows, Cc), w)       # [num_head, rows, ncls]
         return out.view(rows_all, self.head_class_num).index_select(0, dest)
 
-    @torch.no_grad()
     def forward(self, idx, segm_tokens, texture_tokens, t=None):
+        """``t`` is ignored, as in the reference.  In training mode, with autograd recording and a parameter that
+        requires grad (the reference's optimize_parameters), the call is ONE autograd node whose backward is the
+        native trainer's (``transformer_train.sampler_node``); otherwise the inference path below."""
+        from .vqgan_autograd import recording
+        if recording(self):
+            from .transformer_train import sampler_node
+            return sampler_node(self, idx, segm_tokens, texture_tokens)
         logits = self.forward_logits(idx, segm_tokens, texture_tokens)
         # reference returns a list of num_head tensors [B, T, head_class_num] (:271-273)
         return [logits[:, :, i, :] for i in range(self.num_head)]
