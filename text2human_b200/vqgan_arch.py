@@ -426,7 +426,10 @@ class Decoder(nn.Module):
     def forward(self, z, bot_h=None):
         self.last_z_shape = z.shape
         from . import vqgan_autograd as VA
-        if VA.recording(self, z, bot_h):   # training: trunk node + (norm_out, conv_out) node
+        # training: trunk node + (norm_out, conv_out) node.  A bot_h that requires grad takes the nodes in eval mode
+        # too: with fix_decoder the reference never calls decoder.train() and back-propagates through the eval-mode
+        # decoder into bot_h (no BatchNorm, dropout 0: both modes compute the same)
+        if VA.recording(self, z, bot_h) or (bot_h is not None and bot_h.requires_grad and torch.is_grad_enabled()):
             return VA.decoder_forward(self, z, bot_h)
         with torch.no_grad():
             bh = ops.nchw_to_nhwc(bot_h) if bot_h is not None else None
@@ -484,10 +487,13 @@ class DecoderRes(nn.Module):
         self.last_z_shape = torch.Size((z.shape[0], z.shape[3], z.shape[1], z.shape[2]))
         return self._trunk(_conv_in_nhwc(self.conv_in, z))
 
-    @torch.no_grad()
     def forward(self, z):
         self.last_z_shape = z.shape
-        return ops.nhwc_to_nchw(self._trunk(_conv_in_nchw(self.conv_in, z)))
+        from . import vqgan_autograd as VA
+        if VA.recording(self, z):          # training: one autograd node (conv_in + mid) with the hand-written backward
+            return VA.decoder_res_forward(self, z)
+        with torch.no_grad():
+            return ops.nhwc_to_nchw(self._trunk(_conv_in_nchw(self.conv_in, z)))
 
 
 # ----------------------------------------------------------------------------
@@ -682,12 +688,18 @@ class VectorQuantizerSpatialTextureAware(_TextureQuantizerBase):
         r["ids"] = ids
         return r
 
-    @torch.no_grad()
     def forward(self, z, segm_map, temp=None, rescale_logits=False, return_logits=False):
         _check_gumbel_args(temp, rescale_logits, return_logits)
-        r = self.forward_nhwc(ops.nchw_to_nhwc(z), segm_map, want_nchw=True)
-        # unlike the top quantizer, the reference returns the continual indices flat here (:460)
-        return r["zq_nchw"], r["loss"], (None, r["idx_cont"].reshape(-1), list(r["idx_list"].unbind(0)))
+        ps = self.spatial_size
+        if z.dim() != 4 or z.shape[2] % ps or z.shape[3] % ps:
+            raise ValueError(f"latent {tuple(z.shape)}: H and W must be multiples of the patch size {ps}")
+        from . import vqgan_autograd as VA
+        if VA.recording(self, z):          # training: straight-through + codebook-loss gradients
+            return VA.quantizer_spatial_forward(self, z, segm_map)
+        with torch.no_grad():
+            r = self.forward_nhwc(ops.nchw_to_nhwc(z), segm_map, want_nchw=True)
+            # unlike the top quantizer, the reference returns the continual indices flat here (:460)
+            return r["zq_nchw"], r["loss"], (None, r["idx_cont"].reshape(-1), list(r["idx_list"].unbind(0)))
 
     @torch.no_grad()
     def get_codebook_entry(self, indices_list, segm_map, shape, nhwc=False):

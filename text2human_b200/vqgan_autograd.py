@@ -19,6 +19,7 @@ from . import conv_grad as G
 from . import ops
 from . import vqgan_train as VT
 from .flat_params import ConvP
+from .vqgan_bottom_train import RES_LEVEL
 
 
 # ----------------------------------------------------------------------------
@@ -302,29 +303,121 @@ class _DecTailFn(torch.autograd.Function):
         return (None,) + tuple(_unscale(grads, s))
 
 
+def _upper_modules(dec):
+    """the trunk above the residual point: conv_in, mid and the levels from the top down to RES_LEVEL"""
+    return [dec.conv_in, dec.mid] + [dec.up[i] for i in range(RES_LEVEL, dec.num_resolutions)]
+
+
+class _DecTrunkResFn(torch.autograd.Function):
+    """the trunk with the hierarchy residual: upper part (conv_in, mid, levels down to RES_LEVEL) -> + bot_h -> lower
+    part (levels RES_LEVEL-1 .. 0).  The gradient leaving the lower part is d bot_h; the upper part's backward runs
+    only when one of its parameters or z needs a gradient (the reference fills .grad of conv_in, mid and up.4 although
+    its Adam never steps them; quant_top comes from no_grad)."""
+
+    @staticmethod
+    def forward(ctx, dec, z, bot_h, *params):
+        host = _Host(want_grads=True)
+        upper_ids = {id(p) for m in _upper_modules(dec) for p in m.parameters()}
+        need = ctx.needs_input_grad
+        ctx.run_upper = need[1] or any(n for (p, _), n in zip(_trunk_params(dec), need[3:]) if id(p) in upper_ids)
+        inl = VT.ConvL(host, dec.conv_in, "k3", need_dx=need[1])
+        upper = VT.Seq(VT.mid_layers(host, dec.mid) + VT.decoder_up_layers(host, dec, dec.num_resolutions - 1,
+                                                                            bottom_level=RES_LEVEL))
+        lower = VT.Seq(VT.decoder_up_layers(host, dec, RES_LEVEL - 1))
+        with torch.no_grad():
+            h = upper.fwd(inl.fwd(VT.Act(ops.nchw_to_nhwc(z.detach().float().contiguous()))))
+            # the statistics of the sum are not known: the first level-3 block computes them
+            h = lower.fwd(VT.Act(ops.add_inplace(h.x, ops.nchw_to_nhwc(bot_h.detach().float().contiguous()))))
+        ctx.host, ctx.layers, ctx.dec = host, (inl, upper, lower), dec
+        dec.__dict__["_t2h_tail_stats"] = (h.x.data_ptr(), h.stats)
+        return h.x
+
+    @staticmethod
+    def backward(ctx, dh):
+        inl, upper, lower = ctx.layers
+        s = _pow2_scale(dh, target=1.0)
+        dz = None
+        with torch.no_grad(), _Replayable(ctx.host, [inl, upper, lower]) as rp:
+            g = lower.bwd(VT.Grad((dh * s).contiguous()))
+            dbot = ops.nhwc_to_nchw(g.g)
+            if ctx.run_upper:
+                g = inl.bwd(upper.bwd(g))
+                if g is not None:
+                    dz = ops.nhwc_to_nchw(g.g)
+            grads = rp.take([ctx.host.space.grad_of(p, m) if n else None
+                             for (p, m), n in zip(_trunk_params(ctx.dec), ctx.needs_input_grad[3:])])
+        out = _unscale([dz, dbot] + grads, s)
+        return (None,) + tuple(out)
+
+
 def decoder_forward(dec, z, bot_h=None):
-    assert bot_h is None, "training through the hierarchy residual is not on the config-5 path"
     assert not dec.give_pre_end
-    h = _DecTrunkFn.apply(dec, z, *[p for p, _ in _trunk_params(dec)])
+    if bot_h is None:
+        h = _DecTrunkFn.apply(dec, z, *[p for p, _ in _trunk_params(dec)])
+    else:
+        if dec.num_resolutions <= RES_LEVEL:
+            raise ValueError(f"a decoder of {dec.num_resolutions} levels has no level {RES_LEVEL} to add bot_h after")
+        h = _DecTrunkResFn.apply(dec, z, bot_h, *[p for p, _ in _trunk_params(dec)])
     return _DecTailFn.apply(dec, h, dec.norm_out.weight, dec.norm_out.bias, dec.conv_out.weight, dec.conv_out.bias)
 
 
 # ----------------------------------------------------------------------------
-# VectorQuantizerTexture (straight-through + legacy-beta codebook loss, vqgan_arch.py:270-281)
+# DecoderRes (conv_in -> mid: the bottom level's bot_h, reference vqgan_arch.py:1136-1151)
 # ----------------------------------------------------------------------------
+class _DecResFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, dres, z, *params):
+        host = _Host(want_grads=True)
+        inl = VT.ConvL(host, dres.conv_in, "k3", need_dx=ctx.needs_input_grad[1])
+        body = VT.Seq(VT.mid_layers(host, dres.mid))
+        with torch.no_grad():
+            h = body.fwd(inl.fwd(VT.Act(ops.nchw_to_nhwc(z.detach().float().contiguous()))))
+        ctx.host, ctx.layers, ctx.dres = host, (inl, body), dres
+        return ops.nhwc_to_nchw(h.x)
+
+    @staticmethod
+    def backward(ctx, dh):
+        inl, body = ctx.layers
+        s = _pow2_scale(dh, target=1.0)
+        with torch.no_grad(), _Replayable(ctx.host, [inl, body]) as rp:
+            g = inl.bwd(body.bwd(VT.Grad(ops.nchw_to_nhwc((dh * s).contiguous()))))
+            dz = ops.nhwc_to_nchw(g.g) if g is not None else None
+            grads = rp.take([ctx.host.space.grad_of(p, m) for p, m in _params_with_owner(ctx.dres)])
+        return (None,) + tuple(_unscale([dz] + grads, s))
+
+
+def decoder_res_forward(dres, z):
+    return _DecResFn.apply(dres, z, *[p for p, _ in _params_with_owner(dres)])
+
+
+# ----------------------------------------------------------------------------
+# the texture quantizers (straight-through + legacy-beta codebook loss): VectorQuantizerTexture on single positions
+# (vqgan_arch.py:270-281) and VectorQuantizerSpatialTextureAware on ps x ps patches (:449-458)
+# ----------------------------------------------------------------------------
+def _books_selected(ids, n_books):
+    """which codebooks some position selects: one device->host read of ``n_books`` flags"""
+    flat = ids.reshape(-1).long()
+    flat = flat[(flat >= 0) & (flat < n_books)]
+    return (torch.bincount(flat, minlength=n_books)[:n_books] > 0).tolist()
+
+
 class _VQTexFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, z, segm_map, *weights):
+    def forward(ctx, q, ps, z, segm_map, *weights):
         with torch.no_grad():
             zh = ops.nchw_to_nhwc(z.detach().float().contiguous())
             cb = torch.stack([w.detach().float() for w in weights]).contiguous()
             B, H, W, _ = zh.shape
-            ids = ops.mask_to_ids(segm_map, H, W)
-            r = ops.vq_search(zh, cb, ids, cont_stride=1024)
+            ids = ops.mask_to_ids(segm_map, H // ps, W // ps)
+            # the reference hard-codes 1024 as the top quantizer's continual-index stride (:262), n_e for the patches
+            r = ops.vq_search(zh, cb, ids, ps=ps, cont_stride=1024 if ps == 1 else q.n_e)
             loss = ((1.0 + q.beta) * r["sqerr"][0] / zh.numel()).to(torch.float32)
-        ctx.q, ctx.saved_vq = q, (zh, cb, r["idx"], ids)
+        ctx.q, ctx.ps, ctx.saved_vq = q, ps, (zh, cb, r["idx"], ids)
         idx_list = r["idx_list"]
         ctx.mark_non_differentiable(r["idx_cont"], idx_list)
+        if ps != 1 and not ctx.needs_input_grad[2]:
+            # z_q = z + (z_q - z).detach() (:458) carries a gradient only when z does
+            ctx.mark_non_differentiable(r["zq_nchw"])
         return r["zq_nchw"], loss, r["idx_cont"], idx_list
 
     @staticmethod
@@ -332,19 +425,36 @@ class _VQTexFn(torch.autograd.Function):
         zh, cb, idx, ids = ctx.saved_vq
         nel = zh.numel()
         dl = float(dloss) if dloss is not None else 0.0
+        # legacy: loss = mean((zq.detach()-z)^2) + beta*mean((zq-z.detach())^2); otherwise beta weighs the z term
+        w_z, w_e = (1.0, ctx.q.beta) if ctx.q.legacy else (ctx.q.beta, 1.0)
+        cz, ce = 2.0 * w_z * dl / nel, 2.0 * w_e * dl / nel
         with torch.no_grad():
             s = _pow2_scale(dzq) if dzq is not None else 1.0
             dzq_h = ops.nchw_to_nhwc((dzq * s).contiguous()) if dzq is not None else None
             dcb = torch.zeros_like(cb)
-            dz = ops.vq_bwd(zh, cb, idx, ids, dzq_h, dcb, 2.0 * dl * s / nel, 2.0 * ctx.q.beta * dl * s / nel)
+            if ctx.ps == 1:
+                dz = ops.vq_bwd(zh, cb, idx, ids, dzq_h, dcb, cz * s, ce * s)
+            else:
+                dz = ops.vq_bwd_patch(zh, cb, idx, ids, dzq_h, dcb, cz * s, ce * s, ps=ctx.ps)
             dzn = ops.nhwc_to_nchw(dz)
         grads = _unscale([dzn, dcb], s)
-        return (None, grads[0], None) + tuple(grads[1].unbind(0))
+        books = list(grads[1].unbind(0))
+        if ctx.ps != 1:
+            # the reference only looks up embedding_list[k] when some patch selects book k (:416): the others keep
+            # .grad None, so that torch.optim.Adam skips them instead of moving them by their first moment
+            books = [g if used else None for g, used in zip(books, _books_selected(ids, len(books)))]
+        return (None, None, grads[0], None) + tuple(books)
 
 
 def quantizer_texture_forward(q, z, segm_map):
-    zq, loss, cont, lst = _VQTexFn.apply(q, z, segm_map, *[e.weight for e in q.embedding_list])
+    zq, loss, cont, lst = _VQTexFn.apply(q, 1, z, segm_map, *[e.weight for e in q.embedding_list])
     return zq, loss, (None, cont, list(lst.unbind(0)))
+
+
+def quantizer_spatial_forward(q, z, segm_map):
+    """-> (z_q, loss, (None, idx_cont flat, 18 index maps)) as VectorQuantizerSpatialTextureAware.forward"""
+    zq, loss, cont, lst = _VQTexFn.apply(q, q.spatial_size, z, segm_map, *[e.weight for e in q.embedding_list])
+    return zq, loss, (None, cont.reshape(-1), list(lst.unbind(0)))
 
 
 # ----------------------------------------------------------------------------

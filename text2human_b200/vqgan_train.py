@@ -408,11 +408,11 @@ def mid_layers(tr, mid):
     return [ResL(tr, mid.block_1), AttnL(tr, mid.attn_1), ResL(tr, mid.block_2)]
 
 
-def decoder_up_layers(tr, dec, top_level):
-    """the decoder's levels ``top_level`` down to 0 (blocks, attention, the upsample of every level but 0), in
-    forward order"""
+def decoder_up_layers(tr, dec, top_level, bottom_level=0):
+    """the decoder's levels ``top_level`` down to ``bottom_level`` (blocks, attention, the upsample of every level but
+    0), in forward order"""
     body = []
-    for i_level in reversed(range(top_level + 1)):
+    for i_level in reversed(range(bottom_level, top_level + 1)):
         lvl = dec.up[i_level]
         for i_block in range(dec.num_res_blocks + 1):
             body.append(ResL(tr, lvl.block[i_block]))
