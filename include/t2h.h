@@ -181,6 +181,14 @@ int t2h_debug_read(long long* out, int n);
  * channel padding.  Entry of Encoder/Decoder.forward (vqgan_arch.py:899,1008). */
 int t2h_nchw_to_planes(const float* x, void* out, int n, int c, int h, int w,
                        int c_pad, int terms, t2h_stream_t stream);
+/* The fp32 NCHW gradient [N,C,H,W] of a 1x1 conv's output (torch's logit gradient at FCNHead.conv_seg,
+ * fcn_arch.py:80-86) -> fp16 planes NHWC [terms][N][H][W][c_pad] of scale*x (pad channels 0) and
+ * sums[c] = sum over N,H,W of scale*x[.,c,.,.] for c < c_pad (0 for pad channels), the conv's bias gradient, added
+ * in an order fixed by the shape (bitwise reproducible).  c_pad <= 256; work: T2H_NGP_MAX_BLOCKS * c_pad doubles of
+ * scratch. */
+#define T2H_NGP_MAX_BLOCKS 1024
+int t2h_nchw_grad_to_planes(const float* x, void* out, float* sums, double* work, int n, int c, int h, int w,
+                            int c_pad, int terms, float scale, t2h_stream_t stream);
 /* fp32 NHWC [N,H,W,C] -> fp32 NCHW.  Exit of the modules. */
 int t2h_nhwc_to_nchw(const float* x, float* out, int n, int c, int h, int w,
                      t2h_stream_t stream);

@@ -16,6 +16,7 @@ OUT_F32, OUT_PLANES = 0, 1
 BIAS_NONE, BIAS_COL, BIAS_ROW = 0, 1, 2
 ACT_NONE, ACT_GELU, ACT_RELU, ACT_LRELU = 0, 1, 2, 3
 CVT_PLAIN, CVT_UP2X, CVT_S2D, CVT_MAXPOOL2, CVT_BILINEAR2X = 0, 1, 2, 3, 4
+NGP_MAX_BLOCKS = 1024  # T2H_NGP_MAX_BLOCKS: t2h_nchw_grad_to_planes' scratch is this many rows of c_pad doubles
 
 
 class TapGemmParams(C.Structure):
@@ -73,6 +74,7 @@ SIGNATURES = {
     "t2h_tapgemm": (_I, [C.POINTER(TapGemmParams), _P]),
     "t2h_debug_read": (_I, [C.POINTER(C.c_longlong), _I]),
     "t2h_nchw_to_planes": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "t2h_nchw_grad_to_planes": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P]),
     "t2h_nhwc_to_nchw": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "t2h_nchw_to_nhwc": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "t2h_f32_to_planes": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),

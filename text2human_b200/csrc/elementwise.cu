@@ -34,6 +34,59 @@ __global__ void nchw_to_planes_kernel(const float* __restrict__ x, __half* __res
   }
 }
 
+// The gradient torch hands a 1x1 conv's NCHW fp32 output -> the operand planes of its weight / data gradients and
+// the per-channel sums (its bias gradient), in one read of x.  Tiles of kNgpPix pixels of one image are assigned to
+// blocks round-robin (tile = blockIdx.x + k * gridDim.x, a grid fixed by the shape); each block reads a tile along
+// the pixels, transposes it through shared memory, writes the planes of scale*x along the channels and adds each
+// channel's sum over the tile, pixels in order, to a per-thread fp64 sum.  The block's sums go to part[block][c];
+// ngp_sums_kernel adds the blocks in order: the sums do not depend on scheduling.
+constexpr int kNgpPix = 32, kNgpThreads = 256, kNgpMaxBlocks = T2H_NGP_MAX_BLOCKS;
+
+__global__ void __launch_bounds__(kNgpThreads) nchw_grad_planes_kernel(const float* __restrict__ x,
+                                                                        __half* __restrict__ out,
+                                                                        double* __restrict__ part, int C, int HW,
+                                                                        int c_pad, int terms, float scale,
+                                                                        long long n_tiles, long long plane) {
+  extern __shared__ float ngp_tile[];  // [kNgpPix][c_pad + 1]
+  const int ld = c_pad + 1;
+  const int tiles_img = (HW + kNgpPix - 1) / kNgpPix;
+  double acc = 0.0;  // thread c's channel sum (c_pad <= kNgpThreads)
+  for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+    const long long n = t / tiles_img;
+    const int p0 = (int)(t % tiles_img) * kNgpPix;
+    const int np = min(kNgpPix, HW - p0);
+    for (int i = threadIdx.x; i < kNgpPix * c_pad; i += blockDim.x) {
+      const int c = i / kNgpPix, p = i % kNgpPix;
+      ngp_tile[p * ld + c] = (c < C && p < np) ? x[(n * C + c) * HW + p0 + p] * scale : 0.f;
+    }
+    __syncthreads();
+    if (threadIdx.x < C) {
+      for (int p = 0; p < np; ++p) acc += (double)ngp_tile[p * ld + threadIdx.x];
+    }
+    // the tile's planes are one contiguous run of np * c_pad halves; c_pad is even, so pairs stay inside a pixel
+    __half* o = out + (n * HW + p0) * (long long)c_pad;
+    for (int i = 2 * threadIdx.x; i < np * c_pad; i += 2 * blockDim.x) {
+      const int p = i / c_pad, c = i % c_pad;
+      __half h0, l0, h1, l1;
+      split_f16(ngp_tile[p * ld + c], h0, l0);
+      split_f16(ngp_tile[p * ld + c + 1], h1, l1);
+      *reinterpret_cast<__half2*>(o + i) = __halves2half2(h0, h1);
+      if (terms == 2) *reinterpret_cast<__half2*>(o + plane + i) = __halves2half2(l0, l1);
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x < c_pad) part[(long long)blockIdx.x * c_pad + threadIdx.x] = acc;
+}
+
+// sums[c] = part[0][c] + part[1][c] + ... in block order (pad channels get 0)
+__global__ void ngp_sums_kernel(const double* __restrict__ part, int n_blocks, int c_pad, float* __restrict__ sums) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= c_pad) return;
+  double s = 0.0;
+  for (int b = 0; b < n_blocks; ++b) s += part[(long long)b * c_pad + c];
+  sums[c] = (float)s;
+}
+
 // x: [N][C][HW] -> out [N][HW][C]   (fp32)
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, float* __restrict__ out, int C,
                                     int HW) {
@@ -805,6 +858,24 @@ int t2h_nchw_to_planes(const float* x, void* out, int n, int c, int h, int w, in
   dim3 grid(ceil_div(hw, 32), ceil_div(c_pad, 32), n), block(32, 8);
   nchw_to_planes_kernel<<<grid, block, 0, as_stream(stream)>>>(
       x, reinterpret_cast<__half*>(out), c, hw, c_pad, terms, (long long)n * hw * c_pad);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_nchw_grad_to_planes(const float* x, void* out, float* sums, double* work, int n, int c, int h, int w,
+                            int c_pad, int terms, float scale, t2h_stream_t stream) {
+  T2H_CHECK_ARG(x && out && sums && work && n > 0 && c > 0 && h > 0 && w > 0, "nchw_grad_to_planes: bad args");
+  T2H_CHECK_ARG(c_pad >= c && c_pad % 8 == 0 && c_pad <= kNgpThreads,
+                "nchw_grad_to_planes: c_pad=%d must be >= c, a multiple of 8 and <= %d", c_pad, kNgpThreads);
+  T2H_CHECK_ARG(terms == 1 || terms == 2, "nchw_grad_to_planes: terms=%d", terms);
+  const int hw = h * w;
+  const long long tiles = (long long)n * ceil_div(hw, kNgpPix);
+  const int blocks = (int)(tiles < kNgpMaxBlocks ? tiles : kNgpMaxBlocks);
+  const size_t smem = (size_t)kNgpPix * (c_pad + 1) * sizeof(float);
+  nchw_grad_planes_kernel<<<blocks, kNgpThreads, smem, as_stream(stream)>>>(
+      x, reinterpret_cast<__half*>(out), work, c, hw, c_pad, terms, scale, tiles, (long long)n * hw * c_pad);
+  T2H_LAUNCH_OK();
+  ngp_sums_kernel<<<ceil_div(c_pad, 128), 128, 0, as_stream(stream)>>>(work, blocks, c_pad, sums);
   T2H_LAUNCH_OK();
   return T2H_OK;
 }

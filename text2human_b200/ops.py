@@ -565,6 +565,25 @@ def nhwc_to_nchw(x):
     return out
 
 
+def nchw_grad_to_planes(g, c_pad, scale=1.0, terms=None, sums=None):
+    """torch's fp32 NCHW gradient [N,C,H,W] of a 1x1 conv's output -> (fp16 planes [T,N,H,W,c_pad] of scale*g, pad
+    channels zero; fp32 [c_pad] per-channel sums of scale*g, the conv's bias gradient, added in a fixed order and
+    written to ``sums`` when given)"""
+    _need_cuda(g)
+    g = _f32c(g)
+    N, Cc, H, W = g.shape
+    terms = terms or get_terms()
+    out = torch.empty((terms, N, H, W, c_pad), dtype=torch.float16, device=g.device)
+    if sums is None:
+        sums = torch.empty((c_pad,), dtype=torch.float32, device=g.device)
+    assert sums.dtype == torch.float32 and sums.is_contiguous() and sums.numel() == c_pad
+    work = torch.empty((_lib.NGP_MAX_BLOCKS * c_pad,), dtype=torch.float64, device=g.device)
+    _count(1)
+    _lib.check(_lib.load().t2h_nchw_grad_to_planes(_ptr(g), _ptr(out), _ptr(sums), _ptr(work), N, Cc, H, W, c_pad,
+                                                   terms, scale, _stream()))
+    return out, sums
+
+
 def nchw_to_nhwc(x):
     _need_cuda(x)
     x = _f32c(x)

@@ -1,7 +1,8 @@
 """H100-native mirror of the parsing generator of ``SampleFromPoseModel`` (pose + shape attributes -> parsing map,
 ``generate_parsing_map``, reference models/sample_model.py:431-437): ShapeAttrEmbedding
 (models/archs/shape_attr_embedding_arch.py), ShapeUNet (models/archs/unet_arch.py:503-674) and FCNHead
-(models/archs/fcn_arch.py:159-225), inference only (eval-mode BatchNorm, Dropout2d is the identity).
+(models/archs/fcn_arch.py:159-225).  In eval mode (BatchNorm's running statistics, Dropout2d the identity) they run
+the inference path below; in training mode their ``forward``s are the autograd nodes of ``parsing_gen_autograd``.
 
 Same constructor arguments, ``forward`` return structures and ``state_dict`` keys as the reference classes, so
 ``parsing_gen.pth`` (``embedder`` / ``encoder`` / ``decoder``) loads with ``strict=True``.  Arithmetic runs in libt2h:
@@ -66,9 +67,14 @@ class ShapeAttrEmbedding(nn.Module):
                 bad = lo[i] if lo[i] < 0 else hi[i]
                 raise ValueError(f"shape attribute {i} has value {bad}, outside its {n} classes 0..{n - 1}")
 
-    @torch.no_grad()
     def forward(self, attr):
-        assert not self.training, "inference only"
+        if self.training:       # the drop-in training path: one autograd node (parsing_gen_autograd)
+            from .parsing_gen_autograd import shape_attr_embedding_forward
+            return shape_attr_embedding_forward(self, attr)
+        return self._forward_eval(attr)
+
+    @torch.no_grad()
+    def _forward_eval(self, attr):
         self.check_attributes(attr)
         return ops.shape_attr_embed(attr.to(self.fusion[0].weight.device), self._packed())
 
@@ -119,6 +125,9 @@ class ShapeUNet(nn.Module):
         return unet_decode(self.decoder, enc)
 
     def forward(self, x, attr_embedding):
+        if self.training:       # batch-statistics BatchNorm; one autograd node when recording (parsing_gen_autograd)
+            from .parsing_gen_autograd import shape_unet_forward
+            return shape_unet_forward(self, x, attr_embedding)
         return [ops.nhwc_to_nchw(d) for d in self.forward_nhwc(x, attr_embedding)]
 
 
@@ -157,6 +166,9 @@ class FCNHead(nn.Module):
         return ops.conv3x3(y, w, b, taps=ops._TAPS_1)
 
     def forward(self, inputs):
+        if self.training:       # batch-statistics BatchNorm, Dropout2d; one autograd node when recording
+            from .parsing_gen_autograd import fcn_head_forward
+            return fcn_head_forward(self, inputs)
         return ops.nhwc_to_nchw(self.forward_logits(ops.nchw_to_nhwc(inputs[self.in_index])))
 
 

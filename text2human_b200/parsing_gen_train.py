@@ -68,6 +68,12 @@ def embedder_linears(emb):
     return out + [emb.fusion[0], emb.fusion[2]]
 
 
+def dropout2d_mask(B, C, p, device, generator=None):
+    """0/1 [B, C]: the draw of nn.Dropout2d(p) on a [B, C, H, W] input, one bernoulli_(1-p) over B*C values from the
+    same generator, so a seeded run drops the channels the reference drops"""
+    return torch.empty((B, C), device=device).bernoulli_(1.0 - p, generator=generator)
+
+
 # ----------------------------------------------------------------------------
 # the trainer
 # ----------------------------------------------------------------------------
@@ -105,8 +111,7 @@ class ParsingGenTrainer(SingleSpaceTrainer):
 
     def draw_dropout_mask(self, B, generator=None):
         """nn.Dropout2d's draw: one Bernoulli(1-p) per image and channel of the head's ConvModule output"""
-        return torch.empty((B, self.head.channels), device=self.device).bernoulli_(1.0 - self.p_drop,
-                                                                                   generator=generator)
+        return dropout2d_mask(B, self.head.channels, self.p_drop, self.device, generator)
 
     # ---- one step
     def training_step(self, data, dropout_mask=None):

@@ -218,8 +218,9 @@ class UNetL:
             cms += reversed(stage.convs)
         return [m for cm in cms for m in (cm.bns[0], cm.conv)]
 
-    def fwd(self, x, e=None):
-        """x fp32 NHWC [N,H,W,C], e fp32 [N,Ce] or None -> the full-resolution decoder output, fp32 NHWC"""
+    def fwd(self, x, e=None, all_outs=False):
+        """x fp32 NHWC [N,H,W,C], e fp32 [N,Ce] or None -> the full-resolution decoder output, fp32 NHWC (with
+        ``all_outs``: every decoder output, coarsest first, the reference's dec_outs)"""
         enc = []
         for i, stage in enumerate(self.stages):
             src, mode = (x, ops.CVT_PLAIN) if i == 0 else (enc[-1], ops.CVT_MAXPOOL2)
@@ -227,19 +228,24 @@ class UNetL:
             enc.append(stage.fwd(a))
         self.saved.append((x.shape[-1], enc))
         y = enc[-1]
+        outs = [y]
         for i in reversed(range(len(self.dec))):
             y = self.dec[i].fwd(enc[i], y)
-        return y
+            outs.append(y)
+        return outs if all_outs else y
 
-    def bwd(self, d, de=None):
+    def bwd(self, d, de=None, d_coarser=None):
         """d fp32 NHWC gradient of the output; the embedding's gradient is added into ``de`` fp32 [N,Ce] (when
-        ``fwd`` was given ``e``)"""
+        ``fwd`` was given ``e``).  ``d_coarser``: gradients (fp32 NHWC, or None) of the coarser decoder outputs,
+        coarsest first as ``fwd(..., all_outs=True)`` returns them, each added where the backward reaches its output"""
         c0, enc = self.saved.pop()
         c_e = 0 if de is None else de.shape[1]
         d_skip = []
-        for blk in self.dec:
+        for j, blk in enumerate(self.dec):
             s, d = blk.bwd(d)
             d_skip.append(s)
+            if d_coarser is not None and d_coarser[len(self.dec) - 1 - j] is not None:
+                ops.add_inplace(d, d_coarser[len(self.dec) - 1 - j])
         for i in reversed(range(len(self.stages))):
             da = self.stages[i].bwd(d)
             if i > 0:

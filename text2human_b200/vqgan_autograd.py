@@ -166,16 +166,22 @@ class _Replayable:
             ly.saved = saved
 
     def take(self, grads):
-        out = [g.clone() if g is not None else None for g in grads]
-        sp = self.host.space
-        for cp in sp.convs.d.values():
-            if cp.gw is not None:
-                cp.gw.zero_()
-            if cp.gb is not None:
-                cp.gb.zero_()
-        for buf in sp.gbuf.values():
-            buf.zero_()
-        return out
+        return take_grads(self.host, grads)
+
+
+def take_grads(host, grads):
+    """copies of ``grads`` (views of ``host``'s gradient buffers) for autograd, which may keep them as ``.grad``; the
+    buffers are zeroed for the next backward of the same graph"""
+    out = [g.clone() if g is not None else None for g in grads]
+    sp = host.space
+    for cp in sp.convs.d.values():
+        if cp.gw is not None:
+            cp.gw.zero_()
+        if cp.gb is not None:
+            cp.gb.zero_()
+    for buf in sp.gbuf.values():
+        buf.zero_()
+    return out
 
 
 # ----------------------------------------------------------------------------
