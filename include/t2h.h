@@ -414,10 +414,14 @@ int t2h_ce_heads(const float* logits, const int64_t* target, const int64_t* head
  * [nh][4] of {pointer, stride_b, stride_t, stride_c} (elements), head k an fp32 [b][t][ncls] tensor, a null pointer
  * standing for zeros.  t2h_head_grads_absmax: *amax = max |g| over all heads (a NaN anywhere gives NaN).
  * t2h_head_grads_to_planes: fp16 planes out[terms][b*t][nh*ncls] of scale*g, head k in columns [k*ncls, (k+1)*ncls)
- * -- the operand the heads' weight- and data-gradient GEMMs read */
+ * -- the operand the heads' weight- and data-gradient GEMMs read.  t2h_head_grads_to_planes_sums: the same planes
+ * (the same bits), and sums[k][c] = sum over b, t of scale*g, head k's bias gradient, added in a fixed order: per-tile
+ * fp64 partials into work (b * ceil(t/64) * nh * ncls doubles), then an in-order reduce */
 int t2h_head_grads_absmax(const int64_t* heads, int nh, int b, int t, int ncls, float* amax, t2h_stream_t stream);
 int t2h_head_grads_to_planes(const int64_t* heads, int nh, int b, int t, int ncls, float scale, int terms, void* out,
                              t2h_stream_t stream);
+int t2h_head_grads_to_planes_sums(const int64_t* heads, int nh, int b, int t, int ncls, float scale, int terms,
+                                  void* out, float* sums, double* work, t2h_stream_t stream);
 /* de[idx[m]] += dx[m] (idx NULL: row index m % t_mod, the positional table) */
 int t2h_embed_bwd(const float* dx, const int64_t* idx, float* de, int64_t rows, int c, int t_mod,
                   t2h_stream_t stream);

@@ -112,6 +112,7 @@ SIGNATURES = {
     "t2h_ce_heads": (_I, [_P, _P, _P, _P, _P, _P, _L, _I, _I, _P]),
     "t2h_head_grads_absmax": (_I, [_P, _I, _I, _I, _I, _P, _P]),
     "t2h_head_grads_to_planes": (_I, [_P, _I, _I, _I, _I, _F, _I, _P, _P]),
+    "t2h_head_grads_to_planes_sums": (_I, [_P, _I, _I, _I, _I, _F, _I, _P, _P, _P, _P]),
     "t2h_embed_bwd": (_I, [_P, _P, _P, _L, _I, _I, _P]),
     "t2h_adam": (_I, [_P, _P, _P, _P, _L, _F, _F, _F, _F, _I, _F, _P]),
     "t2h_conv_wgrad": (_I, [C.POINTER(ConvWgradParams), _P]),

@@ -426,8 +426,13 @@ __global__ void head_grads_absmax_kernel(const HeadGrad* __restrict__ heads, int
 // weight- and data-gradient GEMMs.  One 64 (tokens) x 64 (classes) tile of one head of one image per block.  When the
 // token dimension is the contiguous one (the class-major layout the loss produces) the tile is read along tokens and
 // transposed through shared memory; otherwise it is read along classes.  The output is written along classes.
+// With kSums the block also adds each class's 64 values in fp64, in a fixed order, to part[b][token tile][k*ncls + c];
+// head_sums_reduce_kernel adds those partials in order: sum over b, t of scale*g (the heads' bias gradients), the same
+// bits on every call.
+template <bool kSums>
 __global__ void head_grads_to_planes_kernel(const HeadGrad* __restrict__ heads, int nh, int B, int T, int ncls,
-                                            float scale, int terms, __half* __restrict__ out) {
+                                            float scale, int terms, __half* __restrict__ out,
+                                            double* __restrict__ part) {
   __shared__ float tile[64][65];  // [token][class]
   const int k = blockIdx.z % nh, b = blockIdx.z / nh;
   const int t0 = blockIdx.x * 64, c0 = blockIdx.y * 64;
@@ -456,6 +461,27 @@ __global__ void head_grads_to_planes_kernel(const HeadGrad* __restrict__ heads, 
   }
   __syncthreads();
   const long long NK = (long long)nh * ncls;
+  if constexpr (kSums) {
+    __shared__ double colpart[8][64];
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int c = tx + 32 * j;
+      double acc = 0.0;
+      for (int i = ty; i < 64; i += 8) acc += (double)tile[i][c];
+      colpart[ty][c] = acc;
+    }
+    __syncthreads();
+    if (ty == 0) {
+      double* dst = part + ((long long)b * gridDim.x + blockIdx.x) * NK + (long long)k * ncls;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int c = tx + 32 * j;
+        double acc = 0.0;
+        for (int r = 0; r < 8; ++r) acc += colpart[r][c];
+        if (c0 + c < ncls) dst[c0 + c] = acc;
+      }
+    }
+  }
   const long long plane = (long long)B * T * NK;
   const bool vec = (ncls & 1) == 0;  // every column pair then starts at an even offset
   for (int i = ty; i < 64; i += 8) {
@@ -477,6 +503,16 @@ __global__ void head_grads_to_planes_kernel(const HeadGrad* __restrict__ heads, 
       }
     }
   }
+}
+
+// sums[j] = sum over the rows of part[row][j] in row order (fp64), rounded once to fp32
+__global__ void head_sums_reduce_kernel(const double* __restrict__ part, int rows, long long n,
+                                        float* __restrict__ sums) {
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  double s = 0.0;
+  for (int r = 0; r < rows; ++r) s += part[(long long)r * n + j];
+  sums[j] = (float)s;
 }
 
 // dE[idx[m]] += dx[m]  (embedding backward; also the positional table with idx = m % T)
@@ -676,9 +712,25 @@ int t2h_head_grads_to_planes(const int64_t* heads, int nh, int b, int t, int ncl
   T2H_CHECK_ARG(terms == 1 || terms == 2, "head_grads_to_planes: terms=%d", terms);
   T2H_CHECK_ARG((long long)nh * b <= 65535, "head_grads_to_planes: too many heads x images");
   dim3 grid(ceil_div(t, 64), ceil_div(ncls, 64), nh * b), block(32, 8);
-  head_grads_to_planes_kernel<<<grid, block, 0, as_stream(stream)>>>(reinterpret_cast<const HeadGrad*>(heads), nh, b,
-                                                                     t, ncls, scale, terms,
-                                                                     reinterpret_cast<__half*>(out));
+  head_grads_to_planes_kernel<false><<<grid, block, 0, as_stream(stream)>>>(
+      reinterpret_cast<const HeadGrad*>(heads), nh, b, t, ncls, scale, terms, reinterpret_cast<__half*>(out), nullptr);
+  T2H_LAUNCH_OK();
+  return T2H_OK;
+}
+
+int t2h_head_grads_to_planes_sums(const int64_t* heads, int nh, int b, int t, int ncls, float scale, int terms,
+                                  void* out, float* sums, double* work, t2h_stream_t stream) {
+  T2H_CHECK_ARG(heads && out && sums && work && nh > 0 && b > 0 && t > 0 && ncls > 0,
+                "head_grads_to_planes_sums: bad args");
+  T2H_CHECK_ARG(terms == 1 || terms == 2, "head_grads_to_planes_sums: terms=%d", terms);
+  T2H_CHECK_ARG((long long)nh * b <= 65535, "head_grads_to_planes_sums: too many heads x images");
+  cudaStream_t st = as_stream(stream);
+  dim3 grid(ceil_div(t, 64), ceil_div(ncls, 64), nh * b), block(32, 8);
+  head_grads_to_planes_kernel<true><<<grid, block, 0, st>>>(reinterpret_cast<const HeadGrad*>(heads), nh, b, t, ncls,
+                                                            scale, terms, reinterpret_cast<__half*>(out), work);
+  T2H_LAUNCH_OK();
+  const long long n = (long long)nh * ncls;
+  head_sums_reduce_kernel<<<(unsigned)ceil_div64(n, 128), 128, 0, st>>>(work, b * (int)grid.x, n, sums);
   T2H_LAUNCH_OK();
   return T2H_OK;
 }

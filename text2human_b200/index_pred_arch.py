@@ -1,6 +1,7 @@
 """H100-native mirror of the index-prediction networks that sit between the sampler and the decoder in
 ``sample_and_refine``: the UNet guidance encoder (reference models/archs/unet_arch.py:317-481) and the
-18-head FCN decoder (models/archs/fcn_arch.py:228-348), inference only (eval-mode BatchNorm).
+18-head FCN decoder (models/archs/fcn_arch.py:228-348).  Eval mode is the inference path below; in training mode
+``forward`` runs batch-statistics BatchNorm and Dropout2d as one autograd node per net (``index_pred_autograd``).
 
 Same constructor arguments, ``forward`` return structures and ``state_dict`` keys as the reference classes,
 so ``index_pred_net.pth`` (``guidance_encoder`` / ``index_decoder``) loads with ``strict=True``.  The reference
@@ -150,6 +151,10 @@ class UNet(nn.Module):
         return unet_decode(self.decoder, enc)
 
     def forward(self, x):
+        if self.training:
+            # batch-statistics BatchNorm; one autograd node when autograd records (index_pred_autograd)
+            from .index_pred_autograd import unet_forward
+            return unet_forward(self, x)
         return [ops.nhwc_to_nchw(d) for d in self.forward_nhwc(x)]
 
 
@@ -202,6 +207,10 @@ class MultiHeadFCNHead(nn.Module):
         return ops.bmm_nt(a, w1, bias_col=b1)
 
     def forward(self, inputs):
+        if self.training:
+            # batch-statistics BatchNorm and Dropout2d; one autograd node when autograd records (index_pred_autograd)
+            from .index_pred_autograd import heads_forward
+            return heads_forward(self, inputs)
         x = inputs[self.in_index]
         B, _, H, W = x.shape
         lg = self.forward_logits(ops.nchw_to_nhwc(x))                             # [G, B*H*W, ncls]

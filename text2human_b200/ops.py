@@ -422,16 +422,28 @@ def wgrad(dy, x, out, k_split=0, alpha=1.0, accumulate=False):
     return out
 
 
-def bmm_nt(a, b, *, planes_out=False, alpha=1.0, bias_row=None, a_bcast=False, bias_col=None, act=ACT_NONE):
+def bmm_nt(a, b, *, planes_out=False, alpha=1.0, bias_row=None, a_bcast=False, bias_col=None, act=ACT_NONE,
+           b_kn=False, out=None):
     """out[g] = a[g] @ b[g]^T.  a: planes [T,G,M,K] (or [T,1,M,K] with a_bcast);
     b: planes [T,G,N,K]; views with a unit last stride are accepted.
-    -> fp32 [G,M,N] or planes [T,G,M,N].  bias_row fp32 [M] (shared) or bias_col fp32 [G,N] (per group)."""
+    -> fp32 [G,M,N] or planes [T,G,M,N].  bias_row fp32 [M] (shared) or bias_col fp32 [G,N] (per group).
+    ``b_kn``: b is planes [T,G,K,N] (the contraction index is the row of each stored matrix, e.g. a forward weight
+    used for a data gradient), consumed as an MN-major operand: out[g] = a[g] @ b[g], no transposed copy.
+    ``out``: an fp32 [G,M,N] destination with a unit last stride (e.g. the column blocks of a wider matrix)."""
     _need_cuda(a, b)
     T, Ga, M, K = a.shape
-    Tb, G, N, Kb = b.shape
+    if b_kn:
+        Tb, G, Kb, N = b.shape
+    else:
+        Tb, G, N, Kb = b.shape
     assert K == Kb and a.stride(3) == 1 and b.stride(3) == 1
     assert (Ga == G) or (a_bcast and Ga == 1)
-    out = _alloc_out((G, M, N), planes_out, T, a.device)
+    if out is None:
+        out = _alloc_out((G, M, N), planes_out, T, a.device)
+        d_strides = (M * N, 0, N, 1)
+    else:
+        assert not planes_out and out.dtype == torch.float32 and tuple(out.shape) == (G, M, N) and out.stride(2) == 1
+        d_strides = (out.stride(0), 0, out.stride(1), 1)
     a_sn = a.stride(1)
     a_term_imgs = 1 if T == 1 else a.stride(0) // a_sn
     assert T == 1 or a.stride(0) % a_sn == 0
@@ -440,10 +452,32 @@ def bmm_nt(a, b, *, planes_out=False, alpha=1.0, bias_row=None, a_bcast=False, b
              b=b, b_term_g=1, b_groups=Tb, b_sg=b.stride(0), b_groups2=G, b_sg2=b.stride(1), b_batched=1,
              n_out=N, b_sn=b.stride(2),
              taps=_TAPS_1, d=out, d_mode=OUT_PLANES if planes_out else OUT_F32,
-             d_strides=(M * N, 0, N, 1), d_plane=G * M * N,
+             d_strides=d_strides, d_plane=G * M * N,
              bias=bias_row if bias_col is None else bias_col,
              bias_mode=BIAS_ROW if bias_col is None else BIAS_COL,
-             bias_sn=0 if bias_col is None else N, alpha=alpha, act=act)
+             bias_sn=0 if bias_col is None else N, alpha=alpha, act=act, b_mn=1 if b_kn else 0)
+    return out
+
+
+def wgrad_batched(dy, x, out, alpha=1.0):
+    """out[g] = alpha * dy[g]^T @ x[g] over the rows, for every group g in ONE launch (the per-head weight gradients
+    of a batched 1x1 conv).  dy planes [T,G,M,n_out], x planes [T,G,M,n_in]: views with a unit last stride, e.g. the
+    column blocks of [T,M,G*n] planes (``p.view(T, M, G, n).permute(0, 2, 1, 3)``), both consumed as MN-major
+    operands; out fp32 [G,n_out,n_in] with a unit last stride, overwritten."""
+    _need_cuda(dy, x, out)
+    T, G, M, No = dy.shape
+    Ni = x.shape[3]
+    assert tuple(x.shape[:3]) == (x.shape[0], G, M) and x.shape[0] == T
+    assert dy.stride(3) == 1 and x.stride(3) == 1 and out.stride(2) == 1 and tuple(out.shape) == (G, No, Ni)
+    assert out.dtype == torch.float32
+    a_sn = dy.stride(1)
+    assert T == 1 or dy.stride(0) % a_sn == 0
+    a_term_imgs = 1 if T == 1 else dy.stride(0) // a_sn
+    _tapgemm(a=dy, a_term_imgs=a_term_imgs, a_imgs=(T - 1) * a_term_imgs + G, a_bcast=0, n_img=G, H=1, W=No, a_H=1,
+             a_W=No, Cc=M, a_sw=dy.stride(2), a_sh=a_sn, a_sn=a_sn,
+             b=x, b_term_g=1, b_groups=T, b_sg=x.stride(0), b_groups2=G, b_sg2=x.stride(1), b_batched=1, n_out=Ni,
+             b_sn=x.stride(2), taps=_TAPS_1, d=out, d_mode=OUT_F32, d_strides=(out.stride(0), 0, out.stride(1), 1),
+             alpha=alpha, a_mn=1, b_mn=1)
     return out
 
 
@@ -1011,6 +1045,23 @@ def head_grads_to_planes(table, shape, scale=1.0, terms=None):
     _count(1)
     _lib.check(_lib.load().t2h_head_grads_to_planes(_ptr(table), nh, B, T, ncls, scale, terms, _ptr(out), _stream()))
     return out
+
+
+def head_grads_to_planes_sums(table, shape, scale=1.0, terms=None, sums=None):
+    """-> (the planes of ``head_grads_to_planes``, bit for bit; fp32 [nh, ncls] sums over b, t of scale*g, each head's
+    bias gradient, added in a fixed order and written to ``sums`` when given)"""
+    B, T, ncls = shape
+    nh = table.shape[0]
+    terms = terms or get_terms()
+    out = torch.empty((terms, B * T, nh * ncls), dtype=torch.float16, device=table.device)
+    if sums is None:
+        sums = torch.empty((nh, ncls), dtype=torch.float32, device=table.device)
+    assert sums.dtype == torch.float32 and sums.is_contiguous() and sums.numel() == nh * ncls
+    work = torch.empty((B * ((T + 63) // 64) * nh * ncls,), dtype=torch.float64, device=table.device)
+    _count(1)
+    _lib.check(_lib.load().t2h_head_grads_to_planes_sums(_ptr(table), nh, B, T, ncls, scale, terms, _ptr(out),
+                                                         _ptr(sums), _ptr(work), _stream()))
+    return out, sums
 
 
 def embed_bwd_(dE, dx, idx=None, t_mod=0):

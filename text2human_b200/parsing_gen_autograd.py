@@ -8,7 +8,8 @@ batch-statistics BatchNorm, running statistics updated as nn.BatchNorm2d does, D
 ``shape_attr_embed_bwd``.  The nodes hand NCHW fp32 tensors to each other, as the reference's modules do; the head's
 incoming logit gradient becomes conv_seg's operand planes and bias gradient in one pass
 (``ops.nchw_grad_to_planes``).  In training mode without recording (``torch.no_grad``) the same forward runs and
-nothing is saved.  The native, faster path for the same step is ``parsing_gen_train.ParsingGenTrainer``.
+nothing is saved.  The native, faster path for the same step is ``parsing_gen_train.ParsingGenTrainer``.  The UNet
+node also serves index_pred_arch's UNet (no embedding; the input gradient when the input requires one).
 """
 import torch
 
@@ -118,7 +119,7 @@ def shape_attr_embedding_forward(emb, attr):
 
 
 # ----------------------------------------------------------------------------
-# ShapeUNet
+# UNet / ShapeUNet
 # ----------------------------------------------------------------------------
 def _unet_layers(ul):
     out = [ul]
@@ -129,23 +130,28 @@ def _unet_layers(ul):
     return out
 
 
-def _unet_run(unet, host, x, e):
+def _unet_run(unet, host, x, e, need_dx):
     """the training-mode forward: -> (UNetL, the five decoder outputs fp32 NHWC, coarsest first)"""
     # the running statistics are updated by a kernel that torch's version counters do not see
     drop_packed_caches(unet)
-    ul = UNetL(host, unet)
+    ul = UNetL(host, unet, need_dx=need_dx)
     B, C, H, W = x.shape
     xh = x.detach().float().reshape(B, H, W, 1) if C == 1 else ops.nchw_to_nhwc(x.detach())
-    return ul, ul.fwd(xh, e.detach().float().contiguous(), all_outs=True)
+    return ul, ul.fwd(xh, None if e is None else e.detach().float().contiguous(), all_outs=True)
 
 
-class _ShapeUNetFn(torch.autograd.Function):
+class _UNetFn(torch.autograd.Function):
+    """The UNet of index_pred_arch (``e`` None) or ShapeUNet (``e`` the attribute embedding) in training mode: returns
+    the five decoder outputs and takes a gradient on any of them.  The gradient of ``x`` is computed and returned when
+    ``x`` requires one; ShapeUNet's embedding always needs stage 0's data gradient."""
+
     @staticmethod
     def forward(ctx, unet, x, e, *params):
         ctx.set_materialize_grads(False)       # a decoder output the loss does not use arrives as None
         host = _Host(want_grads=True)
-        ul, outs = _unet_run(unet, host, x, e)
-        ctx.unet, ctx.host, ctx.ul, ctx.e_shape, ctx.last_shape = unet, host, ul, e.shape, outs[-1].shape
+        ul, outs = _unet_run(unet, host, x, e, need_dx=e is not None or ctx.needs_input_grad[1])
+        ctx.unet, ctx.host, ctx.ul, ctx.last_shape = unet, host, ul, outs[-1].shape
+        ctx.x_shape, ctx.e_shape = x.shape, None if e is None else e.shape
         _stash(ctx, _unet_layers(ul))
         return tuple(ops.nhwc_to_nchw(o) for o in outs)
 
@@ -158,16 +164,30 @@ class _ShapeUNetFn(torch.autograd.Function):
             return (None,) * n_in
         _restore(ctx, _unet_layers(ul))
         s = _pow2_scale(torch.stack([g.detach().abs().amax() for g in gs]), target=1.0)
+        dx = None
         with torch.no_grad():
             nhwc = [ops.nchw_to_nhwc((g * s).contiguous()) if g is not None else None for g in douts]
             last = nhwc[-1]
             if last is None:
                 last = torch.zeros(ctx.last_shape, dtype=torch.float32, device=gs[0].device)
-            de = torch.zeros(ctx.e_shape, dtype=torch.float32, device=gs[0].device)
-            ul.bwd(last, de, d_coarser=nhwc[:-1])
+            de = None if ctx.e_shape is None else torch.zeros(ctx.e_shape, dtype=torch.float32, device=gs[0].device)
+            da = ul.bwd(last, de, d_coarser=nhwc[:-1])
+            if ctx.needs_input_grad[1]:
+                C = ctx.x_shape[1]
+                dx = ops.nhwc_to_nchw(da if da.shape[-1] == C else da[..., :C].contiguous())
             grads = take_grads(host, [host.space.grad_of(p, m) for p, m in _params_with_owner(unet)])
-        out = _unscale([de] + grads, s)
-        return (None, None, out[0] if ctx.needs_input_grad[2] else None) + tuple(out[1:])
+        dx, de, *out = _unscale([dx, de] + grads, s)
+        return (None, dx, de if ctx.needs_input_grad[2] else None) + tuple(out)
+
+
+def unet_node_forward(unet, x, e=None):
+    """a UNet (``e`` None) or ShapeUNet in training mode: -> the five decoder outputs NCHW, coarsest first; one
+    autograd node when autograd records, else the same forward (batch statistics, running statistics updated)"""
+    if _recording(unet, x, e):
+        return list(_UNetFn.apply(unet, x, e, *unet.parameters()))
+    with torch.no_grad():
+        _, outs = _unet_run(unet, _Host(want_grads=False), x, e, need_dx=False)
+        return [ops.nhwc_to_nchw(o) for o in outs]
 
 
 def shape_unet_forward(unet, x, e):
@@ -176,11 +196,7 @@ def shape_unet_forward(unet, x, e):
     if x.requires_grad and torch.is_grad_enabled():
         raise NotImplementedError("ShapeUNet: no gradient with respect to the pose input (the reference never asks "
                                   "for one)")
-    if _recording(unet, e):
-        return list(_ShapeUNetFn.apply(unet, x, e, *unet.parameters()))
-    with torch.no_grad():
-        _, outs = _unet_run(unet, _Host(want_grads=False), x, e)
-        return [ops.nhwc_to_nchw(o) for o in outs]
+    return unet_node_forward(unet, x, e)
 
 
 # ----------------------------------------------------------------------------

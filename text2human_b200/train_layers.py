@@ -64,11 +64,16 @@ class ConvModuleL(Layer):
     ``fwd`` takes the conv's operand planes (space-to-depth planes for "k4s2"); ``bwd`` the fp32 NHWC gradient of the
     output and returns the operand's fp32 gradient (None without ``need_dx``), or with ``split`` the gradients of its
     first ``split`` channels and of the rest, one data-gradient launch each.  ``bwd(..., want_params=False)``
-    computes the data gradient alone: no parameter gradient, nothing reported ``done``."""
+    computes the data gradient alone: no parameter gradient, nothing reported ``done``.
 
-    def __init__(self, tr, conv, bns, kind, act, need_dx=True):
+    With several BatchNorms, ``bind_stats=True`` re-points their running statistics at views of one buffer each (the
+    native trainer's stacked heads, built once); with ``bind_stats=False`` the layer works on gathered copies and every
+    ``fwd`` writes the updated statistics back into each BatchNorm's own buffers (a layer built per forward call)."""
+
+    def __init__(self, tr, conv, bns, kind, act, need_dx=True, bind_stats=True):
         super().__init__(tr)
         self.conv, self.bns, self.kind, self.act, self.need_dx = conv, tuple(bns), kind, act, need_dx
+        self.bind_stats = bind_stats
         bn0 = self.bns[0]
         assert getattr(conv, "bias", None) is None
         assert all(bn.eps == bn0.eps and bn.momentum == bn0.momentum and bn.momentum is not None
@@ -88,6 +93,8 @@ class ConvModuleL(Layer):
             self.rmean = torch.cat([bn.running_mean.float() for bn in self.bns]).contiguous()
             self.rvar = torch.cat([bn.running_var.float() for bn in self.bns]).contiguous()
             self.nbt = torch.stack([bn.num_batches_tracked for bn in self.bns]).contiguous()
+        if not bind_stats:
+            return
         for k, bn in enumerate(self.bns):
             bn.running_mean = self.rmean[k * C:(k + 1) * C]
             bn.running_var = self.rvar[k * C:(k + 1) * C]
@@ -114,6 +121,12 @@ class ConvModuleL(Layer):
         st = ops.norm_stats(pre, C, n=1)
         ops.bn_update_running(st, self.rmean, self.rvar, pre.numel() // C, self.momentum)
         self.nbt += 1
+        if len(self.bns) > 1 and not self.bind_stats:
+            with torch.no_grad():
+                n = self.bns[0].num_features
+                torch._foreach_copy_([bn.running_mean for bn in self.bns], list(self.rmean.split(n)))
+                torch._foreach_copy_([bn.running_var for bn in self.bns], list(self.rvar.split(n)))
+                torch._foreach_copy_([bn.num_batches_tracked for bn in self.bns], list(self.nbt.unbind(0)))
         if out == "planes" and drop is None:
             y = ops.norm_apply(pre, st, gamma, beta, act=self.act, groups=C, eps=self.eps, n=1)
         else:
@@ -237,7 +250,9 @@ class UNetL:
     def bwd(self, d, de=None, d_coarser=None):
         """d fp32 NHWC gradient of the output; the embedding's gradient is added into ``de`` fp32 [N,Ce] (when
         ``fwd`` was given ``e``).  ``d_coarser``: gradients (fp32 NHWC, or None) of the coarser decoder outputs,
-        coarsest first as ``fwd(..., all_outs=True)`` returns them, each added where the backward reaches its output"""
+        coarsest first as ``fwd(..., all_outs=True)`` returns them, each added where the backward reaches its output.
+        -> the gradient of stage 0's operand, fp32 NHWC (channel-padded, with the embedding's channels after x's), or
+        None without ``need_dx``"""
         c0, enc = self.saved.pop()
         c_e = 0 if de is None else de.shape[1]
         d_skip = []
@@ -254,6 +269,7 @@ class UNetL:
                                        accumulate=True)
             elif de is not None:
                 ops.maxpool2_bcast_bwd(da, c0, c_e, de=de, pool=False, accumulate=True)
+        return da
 
 
 class SingleSpaceTrainer:

@@ -18,7 +18,7 @@ import torch.nn as nn
 from . import conv_grad as G
 from . import ops
 from . import vqgan_train as VT
-from .flat_params import ConvP
+from .flat_params import ConvP, ConvStack
 from .vqgan_bottom_train import RES_LEVEL
 
 
@@ -40,14 +40,45 @@ class _Convs:
 
 class StandaloneSpace:
     """Builds ``ConvP`` views (tap-major master copy, packed planes, gradient buffers) on demand from a module's own
-    parameters; gradient buffers are fresh zeros per backward."""
+    parameters; gradient buffers are fresh zeros per backward.  A ``ConvStack`` is one conv of ``n*Cout`` outputs
+    gathered from its members' weights, and ``joint`` gathers a group of parameters (the BatchNorms of a stacked
+    ConvModule) into one vector; each member's gradient is handed out in its own shape."""
 
     def __init__(self, want_grads):
         self.want_grads = want_grads
         self.convs = _Convs(self)
         self.gbuf = {}
+        self.members = {}        # member conv of a ConvStack -> (ConvP of the stack, its row slice)
+        self.jview = {}          # id(param) of a joint group -> its slice of the group's gradient
+
+    def _make_stack(self, st):
+        co, ci, k, _ = st.convs[0].weight.shape
+        cp = ConvP()
+        n = co * len(st.convs)
+        cp.mod, cp.k, cp.co, cp.ci, cp.co_p, cp.ci_p = st, k, n, ci, n, ci
+        cp.w = G.oihw_to_master(torch.cat([c.weight.detach() for c in st.convs]))
+        cp.wn, cp.wt = G.weight_planes(cp.w)
+        cp.gw = torch.zeros_like(cp.w) if self.want_grads else None
+        cp.b = cp.gb = None
+        for j, c in enumerate(st.convs):
+            self.members[c] = (cp, slice(j * co, (j + 1) * co))
+        return cp
+
+    def joint(self, params, cols=None):
+        """-> (the parameters gathered into one fp32 vector (or [rows, cols] matrix), a zeroed gradient of that shape)"""
+        shape = (-1,) if cols is None else (-1, cols)
+        p = torch.cat([q.detach().float().reshape(-1) for q in params])
+        g = torch.zeros_like(p)
+        self.gbuf[("joint", id(params[0]))] = g
+        off = 0
+        for q in params:
+            self.jview[id(q)] = g[off:off + q.numel()].view_as(q)
+            off += q.numel()
+        return p.view(shape), g.view(shape)
 
     def _make(self, mod):
+        if isinstance(mod, ConvStack):
+            return self._make_stack(mod)
         w = mod.weight
         co, ci, k, _ = w.shape
         cp = ConvP()
@@ -74,11 +105,16 @@ class StandaloneSpace:
         """gradient of parameter ``p`` of module ``owner`` in the parameter's own layout"""
         if isinstance(owner, nn.Conv2d):
             cp = self.convs.d.get(owner)
+            if cp is None and owner in self.members:
+                cp, rows = self.members[owner]
+                return G.master_as_oihw(cp.gw[:, rows], rows.stop - rows.start, cp.ci, cp.k)
             if cp is None:
                 return None
             if p is owner.weight:
                 return G.master_as_oihw(cp.gw, cp.co, cp.ci, cp.k)
             return cp.gb[:cp.co]
+        if id(p) in self.jview:
+            return self.jview[id(p)]
         return self.gbuf.get(id(p))
 
     def done(self, mod):
